@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Benchmark of record: multimodal prefill tokens/sec of the MM_LLMs forward (BASELINE.json metric).
 
-  python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path (one rank per GPU under torchrun)
+  python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a path (one rank per GPU under torchrun)
+  python bench.py ... --dump-outputs DIR                   # also write the last timed step's logits (seeded sample) as .npy
   python bench.py --impl reference --gpus N --steps K ...  # the UNMODIFIED reference modeling.py on the host CPUs (oracle/_ref)
 
 Workload (config.workload): BASELINE config 4 — image + audio + text, CLIP ViT-L/14-224 + Whisper-base encoder +
@@ -81,7 +82,7 @@ def synth_inputs(B, L, V, img, mel_T, seed, dtype=torch.bfloat16, pin=True, vide
 
 # ---------------------------------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi sampling during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampling during the timed region (the clocks field of the result line)."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -134,8 +135,25 @@ def load_peaks():
     if os.path.exists(p):
         with open(p) as f:
             d = json.load(f)
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops", 1590.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 6650.0, 1590.0, 1400.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops", 989.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+    return 3350.0, 989.0, 989.0, "H100 SXM data sheet (dense bf16, 700 W; not a measured rate)"
+
+
+def dump_outputs(out_dir: str, logits: "torch.Tensor", n_rows: int = 256) -> None:
+    """Write what the timed path returned in its last step: `logits_last.npy` (B, V) — every sample's last-position
+    logits — and `logits_rows.npy` (n_rows, V) with `logits_rows_index.npy` (n_rows, 2) = (sample, position) of a fixed
+    sample of rows drawn with a seeded generator.  float32; 256 rows of a 32000-word vocabulary are 33 MB."""
+    os.makedirs(out_dir, exist_ok=True)
+    B, T, V = logits.shape
+    g = torch.Generator().manual_seed(0)
+    flat = torch.randperm(B * T, generator=g)[:min(n_rows, B * T)].sort().values
+    idx = torch.stack([flat // T, flat % T], dim=1)
+    rows = logits.reshape(B * T, V)[flat.to(logits.device)]
+    import numpy as np
+
+    np.save(os.path.join(out_dir, "logits_last.npy"), logits[:, -1, :].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "logits_rows.npy"), rows.float().cpu().numpy())
+    np.save(os.path.join(out_dir, "logits_rows_index.npy"), idx.to(torch.float64).numpy())
 
 
 def usable_cores() -> int:
@@ -245,12 +263,15 @@ def cpu_reference_sample(cfgs, hyper, L, steps, warmup, seed=1234, state_dict=No
 def run_train(args, cfgs, hyper, rank, local_rank, world):
     """Secondary line: one TRAINING step (SURVEY.md §8f rank 1) = zero_grad + forward + backward + gradient all-reduce +
     fused AdamW on the cfg4 shape at the reference's micro-batch (train.sh: 4 samples per GPU, fp32 master weights).
-    Weak scaling: per-GPU work is fixed, the data-parallel group grows."""
+    Weak scaling: per-GPU work is fixed, the data-parallel group grows.  Every rank holds a full replica, so what fits one
+    80 GB GPU decides the trainable set: the top `--train-layers` decoder layers (default 8 of 32) are trained together
+    with lm_head, the final norm, the embedding table and every alignment module; the lower layers are frozen (no weight
+    gradient, no AdamW state) and the backward pass runs through them.  Training all 32 layers needs ~112 GB."""
     import torch.distributed as dist
 
     from macaw_llm_b200 import ops
     from macaw_llm_b200.modeling import MM_LLMs, MM_LLMs_Config
-    from macaw_llm_b200.training import FusedAdamW, freeze_like_reference, trainable_parameters
+    from macaw_llm_b200.training import FusedAdamW, freeze_like_reference, freeze_llama_layers, trainable_parameters
 
     clip, whisper, llama = cfgs
     torch.cuda.set_device(local_rank)
@@ -261,6 +282,9 @@ def run_train(args, cfgs, hyper, rank, local_rank, world):
     cfg = MM_LLMs_Config(clip_config=clip, whisper_config=whisper, llm_config=llama, **hyper)
     model = MM_LLMs.build_random(cfg, device=dev, dtype=torch.bfloat16, seed=0)
     freeze_like_reference(model)
+    n_layers = len(model.llm.model.layers)
+    n_train_layers = n_layers if args.train_layers < 0 else min(args.train_layers, n_layers)
+    freeze_llama_layers(model, n_layers - n_train_layers)
     host = synth_inputs(Bl, L, V, clip.vision_config.image_size, 2 * whisper.max_source_positions, 1234 + rank)
     host["labels"] = host["input_ids"].clone()
     inp = {k: (v.to(dev) if isinstance(v, torch.Tensor) else v) for k, v in host.items()}
@@ -350,19 +374,22 @@ def run_train(args, cfgs, hyper, rank, local_rank, world):
     if rank == 0:
         T = L + 16
         n_train = sum(p.numel() for p in params)
-        # 6 FLOP per trainable parameter per token (fwd 2 + bwd 4) + the frozen encoders' / alignment forward
-        tf = (6.0 * n_train * Bl * T + Bl * (162.4e9 + 87.4e9)) / 1e12
+        n_frozen = sum(p.numel() for p in model.llm.parameters() if not p.requires_grad)
+        # 6 FLOP per trainable parameter per token (fwd 2 + bwd 4), 4 per frozen decoder parameter (fwd 2 + data gradient 2)
+        # + the frozen encoders' / alignment forward
+        tf = ((6.0 * n_train + 4.0 * n_frozen) * Bl * T + Bl * (162.4e9 + 87.4e9)) / 1e12
         print(json.dumps({
             "mode": "train", "metric": "multimodal training tokens/sec (img+audio+text->LLaMA, fwd+bwd+all-reduce+AdamW)",
             "value": world * Bl * T / (ms / 1e3), "unit": UNIT, "n_gpus": world, "steps": args.steps,
             "warmup": max(args.warmup, 3), "ms_per_step": ms, "higher_is_better": True, "scaling": "weak", "dtype": "bf16",
             "data": "synthetic",
             "config": {"workload": f"cfg4 shape, micro-batch {Bl}/GPU (train.sh), L={L} -> T={T}, LLaMA-7B + CLIP-L + Whisper-base",
-                       "trainable_params": n_train, "optimizer": "fused AdamW, fp32 master + moments",
+                       "trainable_params": n_train, "trained_decoder_layers": f"top {n_train_layers} of {n_layers}",
+                       "optimizer": "fused AdamW, fp32 master + moments",
                        "submission": "cuda_graph_replay of the whole step" if use_graph else "host_launches",
                        "grad_sync": ("flat bf16 buffer, one NCCL all-reduce per decoder layer on a side stream, overlapped with backward ("
                                      + ("mm_nccl_allreduce" if own_nccl else "torch.distributed") + ")") if world > 1 else "none (1 rank)",
-                       "differentiable_set": "llm.* + the alignment modules of every modality (incl. the table as the alignment attention's keys/values); video_long_self_attention; encoders frozen; MHA attention dropout p=0.1 live (Philox mask regenerated in backward)"},
+                       "differentiable_set": "lm_head, final norm, embed_tokens, the trained decoder layers + the alignment modules of every modality (incl. the table as the alignment attention's keys/values); video_long_self_attention; encoders frozen; MHA attention dropout p=0.1 live (Philox mask regenerated in backward)"},
             "approx_tflops": tf / (ms / 1e3), "gpu_launches": launches, "loss_first_last": [losses[0], losses[-1]],
             "mem_gb": torch.cuda.max_memory_allocated() / 2 ** 30}), flush=True)
     if world > 1:
@@ -431,12 +458,19 @@ def main():
     ap.add_argument("--ddp-graph", type=int, default=1, help="--mode train, N > 1: capture the step incl. the NCCL buckets in a CUDA graph")
     ap.add_argument("--kernel-table", action="store_true", help="--mode train: per-kernel time table of one step on stderr")
     ap.add_argument("--micro-batch", type=int, default=4, help="--mode train: samples per GPU per step (train.sh: 4)")
+    ap.add_argument("--train-layers", type=int, default=8,
+                    help="--mode train: decoder layers trained at the top of the stack (default 8, which fits one 80 GB GPU "
+                         "at micro-batch 4; -1 = all 32, ~112 GB); the rest are frozen, the backward passes through them")
     ap.add_argument("--config", default="cfg4", choices=["cfg4", "cfg5"],
                     help="cfg4 = the benchmark of record (image+audio+text, global batch 32); cfg5 = secondary line: video "
                          "(16 CLIP frames -> 4096 tokens, head_dim-96 self-attention) + audio + text, global batch 16")
     ap.add_argument("--dtype", default=DEFAULT_DTYPE, choices=["bf16", "fp16"],
                     help="storage / tensor-core operand format of the prefill arm (fp32 accumulation either way); the "
                          "reference itself runs fp16 (train.sh --fp16 True)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="prefill: after the timed steps, write what the last timed step returned (float32 .npy files, "
+                         "< 64 MB: every sample's last-position logits and a fixed, seeded sample of logit rows); with "
+                         "several ranks, rank 0 writes its own shard of the global batch (the first B / N samples)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -479,9 +513,9 @@ def main():
         print(json.dumps(line), flush=True)
         return
 
-    # ------------------------------------------------------------------ B200 arm
+    # ------------------------------------------------------------------ GPU arm
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device — the B200 path has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py: no CUDA device — the GPU path has no CPU fallback (use --impl reference for the CPU arm)")
     if args.mode == "train":
         return run_train(args, cfgs, hyper, rank, local_rank, world)
     if args.mode == "decode":
@@ -568,6 +602,8 @@ def main():
     barrier()
     ms = e0.elapsed_time(e1)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, logits)
     t = torch.tensor([ms], device=dev, dtype=torch.float64)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -603,7 +639,7 @@ def main():
             dist.destroy_process_group()
         return
 
-    # ---- live roofline of the dominant kernel (the tcgen05 GEMM): algorithmic FLOPs / CUDA-event time, all launches
+    # ---- live roofline of the dominant kernel (the wgmma GEMM): algorithmic FLOPs / CUDA-event time, all launches
     hbm_peak, tf_burst, tf_sust, peak_src = load_peaks()
     by_tag = {}
     for tag, flops, a, b in prof:
@@ -622,7 +658,7 @@ def main():
         except Exception:
             traffic = None
     roofline = {
-        "kernel": "mm::gemm_bf16_kernel (tcgen05 + TMA), all launches of the step",
+        "kernel": "mm::gemm_bf16_kernel (wgmma + TMA), all launches of the step",
         "bound": "tensor", "achieved": achieved, "peak": tf_sust, "unit": "TFLOP/s", "frac": achieved / tf_sust,
         "peak_source": f"{peak_src} bf16_tflops_sustained (kernel timed inside a long step)", "traffic": traffic,
         "share_of_step": tot_s / (prof_ms / 1e3),
@@ -675,7 +711,7 @@ def main():
         "dtype": args.dtype, "data": "synthetic",
         "config": {"workload": workload, "global_batch": B_global, "per_gpu_batch": B_local, "seq_len": L, "T": T,
                    "parallelism": f"dp{world}", "submission": ("cuda_graph_replay" if use_graphs else "host_launches"),
-                   "l2": "per-step working set (16 GB of weights) >> 126 MB L2; no flush needed"},
+                   "l2": "per-step working set (16 GB of weights) >> 50 MB L2; no flush needed"},
         "clocks": clocks,
         "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                 "result": f"next-token logits (B, V) {args.dtype} read back to pinned host memory (an inference consumer's result)"},

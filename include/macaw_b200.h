@@ -1,5 +1,5 @@
 /*
- * macaw_b200.h — C ABI of libmacaw_b200.so, the sm_100a kernel library behind the MM_LLMs forward hot path.
+ * macaw_b200.h — C ABI of libmacaw_b200.so, the sm_90a kernel library behind the MM_LLMs forward hot path.
  *
  * The reference (lyuchenyang/Macaw-LLM) has no FFI layer of its own: its hot path is Python calling
  * torch / transformers modules (SURVEY.md §8b).  Each entry point below therefore cites the reference
@@ -47,7 +47,7 @@ int32_t mm_get_act_format(void);
  *   alignment MHA in/out projections      modeling.py:986-987, 1007-1008, 1025-1026 -> torch F.multi_head_attention_forward
  *   Conv1d down-samplers, Linear C->E     modeling.py:982-984, 999-1001, 1022-1024
  *   CLIP / Whisper encoder linears, convs  modeling.py:1073, 1082, 1092 -> transformers modeling_clip / modeling_whisper
- * Implementation: persistent, warp-specialised TMA -> tcgen05.mma (TMEM accumulators) kernel.
+ * Implementation: persistent, warp-specialised TMA -> wgmma kernel (register accumulators, two consumer warpgroups).
  */
 enum {
   MM_ACT_NONE = 0,
@@ -93,8 +93,8 @@ typedef struct mm_gemm_args {
   int32_t c_trans; /* 1: C and residual are addressed transposed (C[n][m], row stride ldc), bias is indexed by m, row_scale by n:
                       lets a caller swap the operands (A = weight rows, B = a handful of activation rows) so that thin
                       decode GEMMs fill the 128-row MMA tile with weights (standard epilogue, batch == 1) */
-  /* 16-bit operand formats: 0 = bf16 (default), 1 = fp16 (IEEE half).  A and B must agree: the instruction descriptor has
-   * independent format fields, but sm_100a raises an illegal-instruction fault for f16 x bf16 (measured, round 2).
+  /* 16-bit operand formats: 0 = bf16 (default), 1 = fp16 (IEEE half).  A and B must agree: wgmma takes one input type
+   * for both operands.
    * The alignment chain runs in fp16 (11-bit significand: one stored stage costs 1.4e-4 norm-wise instead of bf16's
    * 1.1e-3) against fp16 COPIES of its weights and of the embedding table (exact conversions of the bf16 values). */
   int32_t a_fp16, b_fp16;
@@ -119,27 +119,27 @@ typedef struct mm_gemm_args {
   int32_t rs_parts;
   float rs_eps;
   /* Stream-K tail (optional; null = plain data-parallel tiles).  When the tile count leaves a partial last wave
-   * (e.g. 272 tiles on 148 SMs), the tail's k-blocks are divided evenly over ALL CTAs; partial fp32 accumulators pass
+   * (e.g. 288 tiles on 132 SMs), the tail's k-blocks are divided evenly over ALL CTAs; partial fp32 accumulators pass
    * through this workspace: 8192 bytes of flags (zero before the first use, self-resetting afterwards) followed by one
-   * 128 x 256 fp32 slot per SM — mm_gemm_streamk_workspace_bytes().  One workspace must not be used by GEMMs running
-   * CONCURRENTLY on different streams.  Ignored for multicast-pair launches and for launches without one full wave of
-   * tiles (the tail pieces run first and hide their hand-over behind the full tiles). */
+   * 128 x 128 fp32 slot per SM — mm_gemm_streamk_workspace_bytes().  One workspace must not be used by GEMMs running
+   * CONCURRENTLY on different streams.  Ignored for launches without one full wave of tiles (the tail pieces run first
+   * and hide their hand-over behind the full tiles). */
   void* sk_workspace;
   int64_t sk_workspace_bytes;
 } mm_gemm_args;
 
 int32_t mm_gemm_fwd(const mm_gemm_args* args, void* stream);
-/* The schedule mm_gemm_fwd would use for `args` on the current device (148 SMs when no device is visible), without
- * touching memory or launching: the host-side decisions — tile width from the cost model, CTA pairs / cta_group::2,
+/* The schedule mm_gemm_fwd would use for `args` on the current device (132 SMs when no device is visible), without
+ * touching memory or launching: the host-side decisions — tile width from the cost model,
  * rasterisation group, stream-K tail — are a pure function of the shapes, strides, alignments and flags.  Operand
  * pointers are only checked for null / alignment, never dereferenced.  Host logic made testable without a GPU
- * (tests/test_gemm_plan.py) and printable per BASELINE shape (tools/gemm_plan.py -> profiles/r2_gemm_schedules.txt). */
+ * (tests/test_gemm_plan.py) and printable per BASELINE shape (tools/gemm_plan.py). */
 typedef struct mm_gemm_schedule {
-  int32_t block_n;             /* tile = 128 x block_n x 64 (pairs: 256 x 256 x 64 per CTA pair) */
-  int32_t pairs;               /* 0 = single CTAs, 1 = multicast pairs of cta_group::1 MMAs, 2 = cta_group::2 pairs */
+  int32_t block_n;             /* tile = 128 x block_n x 64 */
+  int32_t pairs;               /* always 0: every tile runs on one CTA (no CTA-pair schedules on sm_90a) */
   int32_t m_tiles, n_tiles, k_blocks;
-  int64_t units;               /* work units over all batches: tiles, or pair tiles (2 M tiles x 1 N tile) */
-  int32_t workers;             /* units in flight: SMs, or SM pairs */
+  int64_t units;               /* work units over all batches: tiles */
+  int32_t workers;             /* units in flight: SMs */
   int32_t grid;                /* CTAs launched (persistent: <= SM count) */
   int32_t waves;               /* ceil(units / workers) */
   int32_t group_m;             /* rasterisation: M units per L2 group */
@@ -151,10 +151,6 @@ int32_t mm_gemm_plan(const mm_gemm_args* args, mm_gemm_schedule* plan);
 /* Stream-K policy of the process: 0 never, 1 when the saved MMA time exceeds the hand-over cost (default; environment
  * MACAW_B200_GEMM_STREAMK), 2 whenever the schedule allows (tests).  mode < 0 only queries.  Returns the previous mode. */
 int32_t mm_gemm_streamk_mode(int32_t mode);
-/* Pair launches (wide tiles, several waves — the LLaMA GEMMs at batch 32) as ONE cta_group::2 MMA unit (mode 1, default)
- * instead of two cta_group::1 MMAs sharing a multicast B tile (mode 0).  Environment MACAW_B200_GEMM_CG2.  mode < 0 only
- * queries.  Returns the previous mode. */
-int32_t mm_gemm_cg2_mode(int32_t mode);
 /* bytes of mm_gemm_args.sk_workspace on the current device */
 int64_t mm_gemm_streamk_workspace_bytes(void);
 
@@ -182,9 +178,9 @@ typedef struct mm_attn_args {
   const int32_t* key_mask;
   int32_t causal;
   float scale;
-  int32_t impl; /* 0 = tcgen05 kernel (head_dim 64 / 96 / 128); 1 = force the legacy mma.sync kernel (tests only) */
+  int32_t impl; /* 0 = wgmma kernel (head_dim 64 / 96 / 128); 1 = force the mma.sync kernel (tests only) */
   const int32_t* tk_dev; /* NULL, or device int holding the number of valid keys (<= Tk, which then is the capacity of
-                            k / v): lets one captured launch serve a growing KV cache (tcgen05 kernel only) */
+                            k / v): lets one captured launch serve a growing KV cache (wgmma kernel only) */
 } mm_attn_args;
 int32_t mm_attn_fwd(const mm_attn_args* args, void* stream);
 
@@ -231,7 +227,7 @@ int32_t mm_copy_rows(const void* x, int64_t ldx, void* y, int64_t ldy, int32_t r
  *     out[r, :]      = sum_{v < V} P[r, v] * table[v, :]                               (fp16, R x E; "ctx~")
  *     P[r, :]        = softmax over the S = V + 2 keys of { q~[r] . table[v] + row_bias[r] (v < V), extra[r], 0 }
  *     p_sum_real[r]  = sum_{v < V} P[r, v]        p_extra[r] = P of the appended bias_k key
- * ONE persistent kernel: phase 1 streams K-major table tiles through TMA into tcgen05 (S = q~ . table^T) and its
+ * ONE persistent kernel: phase 1 streams K-major table tiles through TMA into wgmma (S = q~ . table^T) and its
  * epilogue writes the un-normalised probabilities once, in fp16 (no fp32 score tensor, no softmax kernel); phase 2
  * streams the SAME table rows as an MN-major operand (O = P' . table) and normalises in its epilogue.  The caller
  * finishes with ctx_h = ctx~_h W_v[h]^T + p_sum_real * b_v[h] + p_extra * bias_v[h] (mm_gemm_fwd with row-scaled biases).
@@ -289,7 +285,7 @@ int32_t mm_argmax_rows(const void* logits, int64_t ld, int32_t rows, int32_t V, 
  * the [32 gate | 32 up]-interleaved product (LlamaMLP modeling.py:139-140). */
 /* Split-K tail of a thin (decode) GEMM: part fp32 [splits][N][ldp] holds W_s x_s^T per K slice (mm_gemm_fwd with the
  * operands swapped, batch = splits, fp32 out); out[m][n] = row_scale[m] * sum_s part[s][n][m] (+ residual[m][n]), bf16.
- * Splitting K lets the 32-tile o_proj / down_proj grids of a decode step cover all 148 SMs (weight streaming). */
+ * Splitting K lets the 32-tile o_proj / down_proj grids of a decode step cover all 132 SMs (weight streaming). */
 int32_t mm_thin_reduce(const float* part, int32_t splits, int32_t N, int32_t M, int32_t ldp, const float* row_scale,
                        const void* residual, int64_t ldr, void* out, int64_t ldo, void* stream);
 /* Fused tail of a split-K thin GEMM — one launch instead of mm_thin_reduce + mm_rope_rows + mm_kv_append /

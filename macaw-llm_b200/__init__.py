@@ -1,4 +1,4 @@
-"""macaw-llm_b200 — B200-native (sm_100a) implementation of the Macaw-LLM `MM_LLMs` forward hot path.
+"""macaw-llm_b200 — H100-native (sm_90a) implementation of the Macaw-LLM `MM_LLMs` forward hot path.
 
 Layout
   csrc/      hand-written CUDA kernels + the C ABI (include/macaw_b200.h)  -> libmacaw_b200.so

@@ -1,4 +1,4 @@
-"""Build libmacaw_b200.so (sm_100a only) in-tree with nvcc.
+"""Build libmacaw_b200.so (sm_90a only) in-tree with nvcc.
 
 The library has no torch dependency: it is plain CUDA behind the C ABI in include/macaw_b200.h, linked against the
 static CUDA runtime so that it can be dlopen()ed on a box without a GPU (symbol checks in the CPU test tier).
@@ -19,7 +19,7 @@ BUILD = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libmacaw_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -107,7 +107,7 @@ def _build_locked(force: bool, verbose: bool) -> str:
         with concurrent.futures.ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             list(ex.map(run, jobs))
     tmp = LIB + f".tmp{os.getpid()}"
-    run([nvcc, "-shared", "-o", tmp] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-ldl"])
+    run([nvcc, "-shared", "-o", tmp] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-ldl"])
     os.replace(tmp, LIB)
     with open(LIB + ".hash.tmp", "w") as f:
         f.write(want + "\n")

@@ -4,14 +4,14 @@
 // table (reference modeling.py:974-975, 986-987, 1007-1008, 1025-1026 -> torch functional.py:6531-6672), in the ABSORBED
 // form of SURVEY.md §7: keys / values are never projected; the per-head query is pushed through W_k (q~ = q_h W_k[h] /
 // sqrt(hd), R = H * Nq rows of width E) and both big contractions stream tiles of the RAW 32000 x 4096 table:
-//     phase 1   S  = q~ . table^T  (R x V, K = E)   table tile = K-major  B operand   (TMA box 64 cols x 256 keys)
+//     phase 1   S  = q~ . table^T  (R x V, K = E)   table tile = K-major  B operand   (TMA box 64 cols x 128 keys)
 //     phase 2   O  = P' . table    (R x E, K = V)   table tile = MN-major B operand   (TMA box 64 cols x 64 keys)
-// — the same row-major table rows serve as "K tile" and "V tile" through two UMMA descriptor flavours, no transpose.
-// Operands are fp16 x fp16 (the table is an exact fp16 copy of the bf16 parameter; sm_100a faults on mixed f16 x bf16).
+// — the same row-major table rows serve as "K tile" and "V tile" through two wgmma descriptor flavours, no transpose.
+// Operands are fp16 x fp16 (the table is an exact fp16 copy of the bf16 parameter; wgmma takes one input type).
 //
 // Why two phases: the flash-style single pass needs the 128 x 4096 fp32 output block (2 MB) resident while all keys
-// stream by; TMEM holds 128 x 512.  Splitting the output columns over CTAs would recompute the scores 8-16x (4.5x the
-// FLOPs of the whole block), so the probabilities are materialised ONCE, in fp16, by the phase-1 epilogue:
+// stream by; a CTA's registers hold 128 x 128.  Splitting the output columns over CTAs would recompute the scores 8-16x
+// (4.5x the FLOPs of the whole block), so the probabilities are materialised ONCE, in fp16, by the phase-1 epilogue:
 //     P'[r, v] = exp2( (s + row_bias) * log2e - rho[r] )          rho = max(extra score, 0) * log2e  (the two synthetic
 // keys' scores: always part of the softmax, so rho is a valid stabiliser that needs no pass over the keys)
 // No fp32 score tensor, no separate softmax kernel, no running-max rescale: rho is constant per row, so phase 2 is a pure
@@ -19,10 +19,11 @@
 // If any real score exceeds rho by more than 2^15 (fp16 range) a flag is raised and phase 1 is re-run with the exact row
 // maxima (collected by atomicMax during the first attempt) — correct for any input, free for ordinary ones.
 //
-// One persistent cooperative launch (148 CTAs, 1 per SM): warp 0 TMA producer, warp 1 single-thread tcgen05.mma issuer,
-// warps 2-9 epilogue (one thread per accumulator row, two warps per TMEM lane quarter); tiles 128 x 256 x 64, 4-stage
-// smem ring, 2 TMEM accumulators.  Phases are separated by a grid-wide barrier (mode 0) or by stream order (mode 1: the
-// same kernel launched three times with the phase selected by an argument).
+// One persistent cooperative launch (one CTA per SM): warp 8 TMA producer, warps 0-7 two consumer warpgroups that issue
+// wgmma (64 rows each, fp32 accumulators in registers), stage the accumulators through shared memory and run the
+// epilogue (one thread per accumulator row, two warps per 32-row quarter); tiles 128 x 128 x 64, 4-stage smem ring.
+// Phases are separated by a grid-wide barrier (mode 0) or by stream order (mode 1: the same kernel launched three times
+// with the phase selected by an argument).
 #include "common.cuh"
 #include "ptx.cuh"
 #include "../../include/macaw_b200.h"
@@ -50,9 +51,10 @@ struct AlignKParams {
   int grid_sync;         // 1: separate the steps by grid-wide barriers (cooperative launch)
 };
 
-constexpr int kAM = 128, kAN = 256, kAK = 64, kAStages = 4;
+constexpr int kAM = 128, kAN = 128, kAK = 64, kAStages = 4;
+constexpr int kALds = kAN + 4;  // staging row stride (floats)
 constexpr uint32_t kAABytes = kAM * kAK * 2, kABBytes = kAN * kAK * 2;
-constexpr size_t kAlignSmem = 1024 + (size_t)kAStages * (kAABytes + kABBytes) + 256;
+constexpr size_t kAlignSmem = 1024 + (size_t)kAStages * (kAABytes + kABBytes) + (size_t)kAM * kALds * 4 + 256;
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kP16Limit = 15.0f;  // P' = 2^t is stored in fp16: t <= 15
 
@@ -74,56 +76,37 @@ __device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
   return v;
 }
 
-__global__ void __launch_bounds__(320, 1)
+__device__ __forceinline__ void align_consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
+__global__ void __launch_bounds__(288, 1)
 align_fused_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmT1,
                    const __grid_constant__ CUtensorMap tmP, const __grid_constant__ CUtensorMap tmT2,
                    const AlignKParams p) {
-  constexpr uint32_t IDESC1 = make_idesc_f16(kAM, kAN, false, false, true, true);  // A, B fp16; B K-major
-  constexpr uint32_t IDESC2 = make_idesc_f16(kAM, kAN, false, true, true, true);   // A, B fp16; B MN-major
-
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;
   uint8_t* sB = smem + kAStages * kAABytes;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sB + kAStages * kABBytes);
+  float* sC = reinterpret_cast<float*>(sB + kAStages * kABBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sC + kAM * kALds);
   uint64_t* empty_bar = full_bar + kAStages;
-  uint64_t* tfull_bar = empty_bar + kAStages;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0 && elect_one()) {
+  if (warp == 8 && elect_one()) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmT1);
     tma_prefetch_desc(&tmP);
     tma_prefetch_desc(&tmT2);
-  }
-  if (warp == 1) {
-    if (elect_one()) {
-      for (int s = 0; s < kAStages; ++s) {
-        mbar_init(&full_bar[s], 1);
-        mbar_init(&empty_bar[s], 1);
-      }
-      for (int s = 0; s < 2; ++s) {
-        mbar_init(&tfull_bar[s], 1);
-        mbar_init(&tempty_bar[s], 8);
-      }
-      fence_mbar_init();
+    for (int s = 0; s < kAStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
     }
-    __syncwarp();
-    tmem_alloc(tmem_slot, 512);
-    tmem_relinquish();
+    fence_mbar_init();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   // pipeline state of each role persists across the steps
   int stage = 0;
   uint32_t ring_phase = 0;
-  int acc = 0;
-  uint32_t acc_phase = 0;
   unsigned epoch = 0;
   const int n_workers = static_cast<int>(gridDim.x), worker = static_cast<int>(blockIdx.x);
 
@@ -136,7 +119,7 @@ align_fused_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
     const int total = p.m_tiles * n_tiles;  // tile index -> m fastest: neighbouring CTAs share the table tile through L2
 
     if (active) {
-      if (warp == 0) {
+      if (warp == 8) {
         // ---------------------------------------------------------------- TMA producer
         if (lane == 0) {  // a fixed lane: the ring state lives in its registers across steps
           if (ph2) asm volatile("fence.proxy.async;" ::: "memory");  // P' was written through the generic proxy
@@ -163,68 +146,78 @@ align_fused_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
           }
         }
         __syncwarp();
-      } else if (warp == 1) {
-        // ---------------------------------------------------------------- MMA issuer
-        if (lane == 0) {
-          const uint32_t idesc = ph2 ? IDESC2 : IDESC1;
-          for (int tile = worker; tile < total; tile += n_workers) {
-            mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + acc * kAN;
+      } else {
+        // ---------------------------------------------------------------- consumers: wgmma, then the epilogue
+        const int wg = warp >> 2;
+        const int q = warp & 3;
+        const int half = warp >> 2;
+        const float* srow = sC + (q * 32 + lane) * kALds;
+        const int flagged = *reinterpret_cast<volatile int*>(p.flag);  // steps 1 / 2: did attempt 0 overflow?
+        const int np = 2 * p.n1_tiles;
+        for (int tile = worker; tile < total; tile += n_workers) {
+          const int m_blk = tile % p.m_tiles, n_blk = tile / p.m_tiles;
+          {
+            float acc[kAN / 2];
+#pragma unroll
+            for (int i = 0; i < kAN / 2; ++i) acc[i] = 0.f;
+            int prev = -1;
             for (int kb = 0; kb < num_k; ++kb) {
               mbar_wait(&full_bar[stage], ring_phase);
-              tc_fence_after();
-              const uint32_t a_addr = smem_u32(sA + stage * kAABytes);
+              const uint32_t a_addr = smem_u32(sA + stage * kAABytes) + wg * 8192;
               const uint32_t b_addr = smem_u32(sB + stage * kABBytes);
               const uint64_t a_desc = make_sdesc_sw128(a_addr, 16, 1024);
               const uint64_t b_desc = ph2 ? make_sdesc_sw128(b_addr, 8192, 1024) : make_sdesc_sw128(b_addr, 16, 1024);
+              wgmma_fence();
+              if (ph2) {
 #pragma unroll
-              for (int kk = 0; kk < kAK / 16; ++kk) {
-                const uint64_t a_k = a_desc + static_cast<uint64_t>(kk * 2);
-                const uint64_t b_k = b_desc + static_cast<uint64_t>(ph2 ? kk * 128 : kk * 2);
-                umma_bf16(d_tmem, a_k, b_k, idesc, (kb | kk) != 0 ? 1u : 0u);
+                for (int kk = 0; kk < kAK / 16; ++kk)
+                  wgmma_ss_n128<true, 0, 1>(acc, a_desc + static_cast<uint64_t>(kk * 2), b_desc + static_cast<uint64_t>(kk * 128), 1u);
+              } else {
+#pragma unroll
+                for (int kk = 0; kk < kAK / 16; ++kk)
+                  wgmma_ss_n128<true, 0, 0>(acc, a_desc + static_cast<uint64_t>(kk * 2), b_desc + static_cast<uint64_t>(kk * 2), 1u);
               }
-              umma_commit(&empty_bar[stage]);
+              wgmma_commit();
+              wgmma_wait<1>();
+              if (prev >= 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[prev]);
+              }
+              prev = stage;
               if (++stage == kAStages) {
                 stage = 0;
                 ring_phase ^= 1;
               }
             }
-            umma_commit(&tfull_bar[acc]);
-            if (++acc == 2) {
-              acc = 0;
-              acc_phase ^= 1;
+            wgmma_wait<0>();
+            fence_regs(acc);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            align_consumer_sync();  // the previous tile's epilogue is done reading the staging tile
+            const int r0 = wg * 64 + q * 16 + (lane >> 2);
+            const int c0 = 2 * (lane & 3);
+#pragma unroll
+            for (int j = 0; j < kAN / 8; ++j) {
+              *reinterpret_cast<float2*>(sC + r0 * kALds + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+              *reinterpret_cast<float2*>(sC + (r0 + 8) * kALds + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
             }
+            align_consumer_sync();
           }
-        }
-        __syncwarp();
-      } else {
-        // ---------------------------------------------------------------- epilogue warps
-        const int q = warp & 3;
-        const int half = (warp - 2) >> 2;
-        const int flagged = *reinterpret_cast<volatile int*>(p.flag);  // steps 1 / 2: did attempt 0 overflow?
-        const int np = 2 * p.n1_tiles;
-        for (int tile = worker; tile < total; tile += n_workers) {
-          const int m_blk = tile % p.m_tiles, n_blk = tile / p.m_tiles;
           const int row = m_blk * kAM + q * 32 + lane;
           const bool row_ok = row < p.R;
           const long long rs = static_cast<long long>(row_ok ? row : 0);
           const float ex2s = p.extra[rs * p.stat_stride] * kLog2e;   // score of the bias_k key (log2 domain)
           float rho = fmaxf(ex2s, 0.0f);                             // the zero key has score 0
           if ((step == 1) || (step == 2 && flagged)) rho = fmaxf(rho, dec_ordered(p.rowmax_u[rs]));
-          const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * kAN;
 
           if (!ph2) {
             const float rb2 = p.row_bias[rs * p.stat_stride] * kLog2e;  // q_h . b_k[h]: added to every real key
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
             __half* prow = p.P + rs * p.ldp;
             float psum = 0.f, tmax = -INFINITY;
 #pragma unroll 1
-            for (int c = half * 4; c < half * 4 + 4; ++c) {
+            for (int c = half * 2; c < half * 2 + 2; ++c) {
               uint32_t r[32];
-              tmem_ld32(taddr + c * 32, r);
-              tmem_ld_wait();
+              stage_ld32(srow + c * 32, r);
               const int key0 = n_blk * kAN + c * 32;
               if (key0 >= p.V) continue;  // warp-uniform
               uint32_t pk[16];
@@ -279,14 +272,11 @@ align_fused_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
               p.p_extra[rs] = e_extra * inv;
               if (p.inv_l_out != nullptr) p.inv_l_out[rs] = inv;
             }
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
             __half* orow = p.out + rs * p.ldo;
 #pragma unroll 1
-            for (int c = half * 4; c < half * 4 + 4; ++c) {
+            for (int c = half * 2; c < half * 2 + 2; ++c) {
               uint32_t r[32];
-              tmem_ld32(taddr + c * 32, r);
-              tmem_ld_wait();
+              stage_ld32(srow + c * 32, r);
               const int col0 = n_blk * kAN + c * 32;
               if (col0 >= p.E || !row_ok) continue;
 #pragma unroll
@@ -299,13 +289,6 @@ align_fused_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
                 *reinterpret_cast<uint4*>(orow + col0 + 8 * i) = u;
               }
             }
-          }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-          if (++acc == 2) {
-            acc = 0;
-            acc_phase ^= 1;
           }
         }
       }
@@ -324,13 +307,6 @@ align_fused_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
       __syncthreads();
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
 }  // namespace mm
@@ -338,7 +314,7 @@ align_fused_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constan
 using namespace mm;
 
 extern "C" int64_t mm_align_workspace_bytes(int32_t R, int32_t V) {
-  // [0,16): barrier counter + overflow flag; then R row maxima (u32); then R x 2*ceil(V/256) partial sums (fp32)
+  // [0,16): barrier counter + overflow flag; then R row maxima (u32); then R x 2*ceil(V/128) partial sums (fp32, kAN = 128)
   if (R <= 0 || V <= 0) return 0;
   const int64_t np = 2LL * ((V + kAN - 1) / kAN);
   return 16 + 4LL * R + 4LL * R * np;
@@ -395,7 +371,7 @@ extern "C" int32_t mm_align_fwd(const mm_align_args* a, void* stream) {
     p.step_lo = lo; p.step_hi = hi; p.grid_sync = coop;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(320);
+    cfg.blockDim = dim3(288);
     cfg.dynamicSmemBytes = kAlignSmem;
     cfg.stream = st;
     cudaLaunchAttribute attr[1];

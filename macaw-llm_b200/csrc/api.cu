@@ -21,7 +21,7 @@ void count_launch(int n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 bool pdl_enabled() {
   static const bool on = []() {
     const char* e = getenv("MACAW_B200_PDL");
-    return e != nullptr && atoi(e) != 0;  // default OFF: measured slower (cfg4 B=4: 27.95 -> 28.8-29.4 ms/step)
+    return e != nullptr && atoi(e) != 0;  // default OFF (opt-in, see common.cuh)
   }();
   return on;
 }
@@ -32,7 +32,7 @@ int num_sms() {
   if (cache[dev] == 0) {
     int n = 0;
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    cache[dev] = n > 0 ? n : 148;
+    cache[dev] = n > 0 ? n : 132;  // H100 SXM when no device is visible
   }
   return cache[dev];
 }
@@ -41,7 +41,7 @@ int num_sms() {
 
 extern "C" {
 const char* mm_last_error(void) { return mm::g_err; }
-int32_t mm_abi_version(void) { return 2; }
+int32_t mm_abi_version(void) { return 3; }
 #ifndef MM_SRC_HASH
 #define MM_SRC_HASH "unknown"
 #endif

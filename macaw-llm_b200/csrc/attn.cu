@@ -5,9 +5,9 @@
 // registers; softmax reductions are warp-shuffle (quad) reductions in fp32; P is re-packed to bf16 in registers and
 // fed straight back to the tensor cores (mma.sync.m16n8k16 bf16, fp32 accumulate).
 //
-// This register-fragment (mma.sync) kernel serves head_dim 96 — the video-long self-attention with its two synthetic
-// keys — and stays selectable (mm_attn_args.impl = 1) as an independent second implementation for the tests.  Head
-// dims 64 / 128 (CLIP, Whisper, LLaMA) run on the tcgen05 kernel in attn_tcgen05.cu, to which mm_attn_fwd dispatches.
+// This register-fragment (mma.sync) kernel stays selectable (mm_attn_args.impl = 1) as an independent second
+// implementation for the tests.  Head dims 64 / 96 / 128 (CLIP, Whisper, video-long, LLaMA) run on the wgmma kernel in
+// attn_wgmma.cu, to which mm_attn_fwd dispatches.
 //
 // Reference call sites replaced: see include/macaw_b200.h (mm_attn_fwd).
 #include "common.cuh"
@@ -267,7 +267,7 @@ static int launch_attn(const AttnKParams& p, cudaStream_t st) {
 }  // namespace mm
 
 namespace mm {
-int attn_tcgen05_dispatch(const mm_attn_args* a, cudaStream_t st);
+int attn_wgmma_dispatch(const mm_attn_args* a, cudaStream_t st);
 }
 using namespace mm;
 
@@ -282,10 +282,10 @@ extern "C" int32_t mm_attn_fwd(const mm_attn_args* a, void* stream) {
   MM_REQUIRE(((uintptr_t)a->q % 16 == 0) && ((uintptr_t)a->k % 16 == 0) && ((uintptr_t)a->v % 16 == 0) &&
                  ((uintptr_t)a->out % 16 == 0),
              "mm_attn_fwd: pointers must be 16-byte aligned");
-  // tcgen05 kernel (attn_tcgen05.cu) for every supported head_dim; impl == 1 forces the mma.sync kernel below (tests)
+  // wgmma kernel (attn_wgmma.cu) for every supported head_dim; impl == 1 forces the mma.sync kernel below (tests)
   if (a->scale > 0.f && a->impl != 1)
-    return attn_tcgen05_dispatch(a, reinterpret_cast<cudaStream_t>(stream));
-  MM_REQUIRE(a->tk_dev == nullptr, "mm_attn_fwd: device-side key length is only supported by the tcgen05 kernel");
+    return attn_wgmma_dispatch(a, reinterpret_cast<cudaStream_t>(stream));
+  MM_REQUIRE(a->tk_dev == nullptr, "mm_attn_fwd: device-side key length is only supported by the wgmma kernel");
   AttnKParams p;
   p.q = (const bf16*)a->q; p.k = (const bf16*)a->k; p.v = (const bf16*)a->v; p.out = (bf16*)a->out;
   p.B = a->B; p.H = a->H; p.Tq = a->Tq; p.Tk = a->Tk;

@@ -65,14 +65,14 @@ inline int ensure_smem_attr(K kern, size_t smem, bool (&flags)[kMaxDevices], con
 }
 
 // 16-bit 4-D TMA map {inner, rows, batch, batch2} (strides in elements), 128B swizzle, box {64, box_rows, 1, 1}
-// (defined in gemm_tcgen05.cu; bf16 and fp16 tensors use the same map — TMA only moves 16-bit elements).
+// (defined in gemm_wgmma.cu; bf16 and fp16 tensors use the same map — TMA only moves 16-bit elements).
 int make_map(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t rows, uint64_t batch, uint64_t batch2, int64_t ld,
              int64_t bs, int64_t bs2, uint32_t box_rows);
 
 // Programmatic dependent launch: kernels call griddep_launch() once their prologue is done (lets the next kernel of the
 // stream start ITS prologue on SMs that free up) and griddep_wait() before their first global-memory access (returns
-// when every predecessor grid has completed and flushed).  The launch attribute is OPT-IN (MACAW_B200_PDL=1): on this
-// workload it measured slower than plain stream order under CUDA-graph replay (B=4: +3 %, B=32: +0.5 %), see DESIGN.md.
+// when every predecessor grid has completed and flushed).  The launch attribute is OPT-IN (MACAW_B200_PDL=1): the
+// persistent one-CTA-per-SM kernels leave no room for the next kernel's CTAs to start early.
 bool pdl_enabled();
 
 template <typename... KArgs, typename... Args>

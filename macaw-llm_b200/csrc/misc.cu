@@ -8,8 +8,6 @@
 
 namespace mm {
 
-constexpr int kSMs = 148;
-
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -744,7 +742,7 @@ __global__ void __launch_bounds__(512) ce_loss_kernel(const bf16* __restrict__ l
 
 static inline int grid_for(long long total, int block) {
   long long g = (total + block - 1) / block;
-  const long long cap = static_cast<long long>(kSMs) * 16;
+  const long long cap = static_cast<long long>(num_sms()) * 16;
   return static_cast<int>(g < cap ? (g > 0 ? g : 1) : cap);
 }
 

@@ -1,6 +1,6 @@
 // HBM-bound kernels of the training step (SURVEY.md §8f rank 1): the backward halves of RMSNorm / SwiGLU / softmax /
 // cross-entropy, the embedding-gradient scatter and the fused AdamW update.  The contractions of the backward pass run on
-// the tcgen05 GEMM (dX = dY W with an MN-major B operand, dW = dY^T X with MN-major A and B operands).
+// the wgmma GEMM (dX = dY W with an MN-major B operand, dW = dY^T X with MN-major A and B operands).
 //
 // Reference: autograd of the vendored LLaMA in /root/reference/modeling.py (LlamaRMSNorm :302-319, LlamaMLP :126-140,
 // LlamaAttention :143-231, shifted CE :597-610) driven by llm_trainer.py:184-188 (compute_loss -> loss.backward()) and the

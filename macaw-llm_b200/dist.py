@@ -1,7 +1,7 @@
 """Multi-GPU plumbing for the forward path: batch sharding and max-over-ranks timing.
 
 The reference distributes with HF Trainer + DeepSpeed ZeRO-3 (train.sh:14-16, configs/deepspeed_config.json); the
-forward itself is embarrassingly parallel over samples (SURVEY.md §8e), so the B200 path runs one full replica per
+forward itself is embarrassingly parallel over samples (SURVEY.md §8e), so the GPU path runs one full replica per
 rank on a contiguous slice of the global batch with NO collective on the data path.  The only cross-rank traffic is
 the scalar reduction used for timing / loss reporting.
 """

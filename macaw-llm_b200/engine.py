@@ -1,4 +1,4 @@
-"""The MM_LLMs forward pass expressed over the sm_100a kernel library (ops.py -> libmacaw_b200.so).
+"""The MM_LLMs forward pass expressed over the sm_90a kernel library (ops.py -> libmacaw_b200.so).
 
 Every arithmetic step of the reference hot path (reference: /root/reference/modeling.py:941-1118 and the torch /
 transformers modules it delegates to) is executed by a hand-written kernel; torch only owns device memory.  The
@@ -7,7 +7,7 @@ engine reads the parameters of an `MM_LLMs` module (modeling.py in this package)
 in-place weight updates are picked up.
 
 Data layout in HBM: activations are bf16, token-major `(tokens, channels)` with the residual stream updated in
-place by GEMM epilogues; all contractions accumulate in fp32 (TMEM / registers); scores of the alignment
+place by GEMM epilogues; all contractions accumulate in fp32 (registers); scores of the alignment
 cross-attention are fp32.
 """
 from __future__ import annotations
@@ -41,13 +41,12 @@ class Engine:
         self._graphs: Dict[tuple, tuple] = {}
         self._decode: Dict[tuple, dict] = {}  # KV buffers + captured decode step per (batch, capacity, device)
         self._side: Dict[str, torch.cuda.Stream] = {}
-        # Whisper tower on a side stream next to the CLIP tower(s).  Measured on B200 (profiles/r2_bench_lines.txt, run 12):
-        # neutral to slightly negative at global batch 32 (+2 ms of 36 ms outside LLaMA: both towers' GEMMs are persistent
-        # one-CTA-per-SM kernels, two of them cannot co-reside, so only launch tails overlap while the late-starting CTAs
-        # stretch the static tile schedule), -0.3 ms at batch 4.  Off by default; kept as a tested option.
+        # Whisper tower on a side stream next to the CLIP tower(s): both towers' GEMMs are persistent one-CTA-per-SM
+        # kernels, two of them cannot co-reside, so only launch tails overlap while the late-starting CTAs stretch the static
+        # tile schedule.  Off by default; kept as a tested option.
         self.overlap_encoders = False
         # Stream-K tail in the LLaMA GEMMs (a partial last wave of tiles is split along K over all SMs): matters at small
-        # per-GPU batch (272 tiles on 148 SMs -> 1.84 waves), a no-op when the tile count fills the waves.
+        # per-GPU batch (e.g. 1088 tiles on 132 SMs -> 8.2 waves), a no-op when the tile count fills the waves.
         self.streamk = True
         self.fused_decode_tails = True  # decode step: one tail kernel per thin GEMM (mm_thin_fused) instead of 2-3 row-wise kernels
         self._sk_ws: Dict[str, torch.Tensor] = {}

@@ -6,7 +6,7 @@
 
 Constructor kwargs, attribute names and `state_dict()` keys match the reference (SURVEY.md §8b), so
 `MM_LLMs(config).load_state_dict(reference_model.state_dict())` is the checkpoint-compatibility mechanism.  The
-modules defined here only HOLD parameters; all arithmetic runs through `engine.Engine` on hand-written sm_100a
+modules defined here only HOLD parameters; all arithmetic runs through `engine.Engine` on hand-written sm_90a
 kernels.  There is no CPU path: calling forward with parameters on the CPU raises.
 """
 from __future__ import annotations

@@ -109,7 +109,7 @@ def gemm_plan(*, M: int, N: int, K: int, batch: int = 1, batch2: int = 1, epi: i
               a_mn_major: bool = False, c_fp32: bool = False, c_trans: bool = False, fp16: bool = False,
               streamk: bool = False) -> dict:
     """The schedule mm_gemm_fwd would pick for a dense, 16-byte-aligned GEMM of this shape (mm_gemm_plan: the host-side
-    dispatch run without touching memory or launching — works without a GPU, where the library assumes 148 SMs).
+    dispatch run without touching memory or launching — works without a GPU, where the library assumes the 132 SMs of an H100 SXM).
     `streamk=True` hands the dispatcher a stream-K workspace, as the LLaMA stack does."""
     lib = _lib.load()
     fake = 1 << 20  # operand addresses are only checked for null / alignment
@@ -214,7 +214,7 @@ def linear_thin(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] =
     return out
 
 
-THIN_SPLITS = 4  # K slices of a thin (decode) GEMM: 32..172-tile grids become 128..688 units on 148 SMs
+THIN_SPLITS = 4  # K slices of a thin (decode) GEMM: 32..172-tile grids become 128..688 units on 132 SMs
 
 
 def linear_thin_splitk(x: torch.Tensor, w: torch.Tensor, *, residual: Optional[torch.Tensor] = None,
@@ -653,7 +653,7 @@ def dropout_mask(rows: int, cols: int, dropout, device) -> torch.Tensor:
 
 def attention_train_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, *, scale: float, causal: bool = False,
                         key_mask: Optional[torch.Tensor] = None, dropout=None) -> torch.Tensor:
-    """Training-mode forward of a DROPOUT attention (the flash kernel has no dropout): S = q k^T (fp32, batched tcgen05
+    """Training-mode forward of a DROPOUT attention (the flash kernel has no dropout): S = q k^T (fp32, batched wgmma
     GEMM), Pd = dropout(softmax(scale S)) (one row-wise kernel, Philox mask), O = Pd v.  Same operand conventions as
     attention_bwd; returns O (B, Tq, H, hd) contiguous."""
     for n, t in (("q", q), ("k", k), ("v", v)):
@@ -684,7 +684,7 @@ def attention_train_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, *, sc
 
 def attention_bwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, do: torch.Tensor, *, scale: float, causal: bool,
                   key_mask: Optional[torch.Tensor] = None, dropout=None):
-    """Backward of mm_attn_fwd composed from tcgen05 GEMMs: S = q k^T and dP = dO v^T (fp32, batched over (b, h)), one
+    """Backward of mm_attn_fwd composed from wgmma GEMMs: S = q k^T and dP = dO v^T (fp32, batched over (b, h)), one
     row-wise softmax-backward kernel (P, dS in bf16), then dV = P^T dO, dK = dS^T q (MN-major A), dQ = dS k.
     q / do (B, Tq, H, hd), k / v (B, Tk, H, hd): bf16 views with unit head-dim stride.  Returns contiguous dq, dk, dv.
     dropout = (p, seed_dev, sid): backward of attention_train_fwd with the same mask (regenerated, not stored)."""

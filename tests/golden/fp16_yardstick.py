@@ -6,11 +6,11 @@ The oracle (oracle/macaw_oracle.py, a restatement of the reference pinned agains
 the same fp16-representable random-init weights and inputs of the FULL-DEPTH model (CLIP ViT-L/14 x24, Whisper-base x6,
 LLaMA-7B x32, V = 32000): once in fp32, once with every activation and matmul in fp16 (torch CPU half kernels, fp32
 accumulation inside a matmul, 16-bit storage between ops — what the reference's `.half()` model does on its GPU).  The
-norm-wise difference is the floor any fp16 implementation of this model sits on; the B200 path's measured error
-(DESIGN.md §6: prefix 6-7e-4, logits 5.1e-3, top-1 agreement 0.98-0.996) is read against it.
+norm-wise difference is the floor any fp16 implementation of this model sits on; the GPU path's measured error
+(tests/test_fp16_gpu.py prints it) is read against it.
 
 Lives under tests/ because it drives the oracle (test infrastructure: only tests/, smoke() and bench.py's CPU arm may).
-Usage: python tests/golden/fp16_yardstick.py [--configs cfg2,cfg4] [--layers 32] [--dtype fp16|bf16] > profiles/r2_fp16_yardstick.txt
+Usage: python tests/golden/fp16_yardstick.py [--configs cfg2,cfg4] [--layers 32] [--dtype fp16|bf16]
 """
 import argparse
 import os

@@ -147,5 +147,27 @@ def main():
     print("[golden] video positional encoding: bit-exact vs reference loop")
 
 
+def live_reference_fixtures():
+    """Outputs of the reference module itself that tests/test_oracle.py and tests/test_wire.py compare against: the
+    tiny model's logits / loss on one seeded batch, and the state-dict layout after `resize_token_embeddings(V + 7)`."""
+    modeling = import_reference()
+    cfg, model, shapes, _ = build_reference(modeling, gen.TINY)
+    inp = gen.make_inputs(gen.TINY, 2, 11, seed=7, modalities=("image", "audio"), pad_tail=2)
+    with torch.no_grad():
+        out = model(inp)
+    np.savez_compressed(os.path.join(HERE, "tiny_live_ref.npz"), logits=out.logits.float().numpy(), loss=float(out.loss))
+    V = cfg.llm_config.vocab_size
+    model.llm.resize_token_embeddings(V + 7)
+    # stored as the difference to the pre-resize layout of tiny_shapes.json (also the reference's): names and shapes
+    after = {k: list(v.shape) for k, v in model.state_dict().items()}
+    delta = {"changed": {k: s for k, s in after.items() if k in shapes and list(shapes[k]) != s},
+             "added": {k: s for k, s in after.items() if k not in shapes},
+             "removed": sorted(k for k in shapes if k not in after)}
+    with open(os.path.join(HERE, "tiny_resized_state.json"), "w") as f:
+        json.dump(delta, f, indent=0, sort_keys=True)
+    print("[golden] live-reference logits / loss and the resized state-dict layout")
+
+
 if __name__ == "__main__":
     main()
+    live_reference_fixtures()

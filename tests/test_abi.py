@@ -83,10 +83,10 @@ def test_integration_md_stub_matches_abi():
     assert ctypes.sizeof(doc) == ctypes.sizeof(_lib.GemmArgs)
 
 
-def test_product_kernels_are_blackwell_native_sass():
+def test_product_kernels_are_hopper_native_sass():
     """Static check of the shipped cubin (cuobjdump, no GPU): the GEMM, flash-attention and fused alignment kernels carry
-    tcgen05.mma (UTCHMMA) + TMA (UTMALDG) + TMEM loads (LDTM); the pair GEMMs carry the cta_group::2 form; mma.sync (HMMA)
-    appears only in the second attention implementation the tests use as a cross-check; nothing spills to local memory."""
+    wgmma (HGMMA) + TMA (UTMALDG) + mbarrier waits (SYNCS); mma.sync (HMMA) appears only in the second attention
+    implementation the tests use as a cross-check; nothing spills to local memory."""
     import shutil
     import sys
 
@@ -108,13 +108,10 @@ def test_product_kernels_are_blackwell_native_sass():
         m = re.match(r"(.+?)\s+((?:\d+\s+){%d}\d+)\s*$" % (len(cols) - 1), l)
         assert m, l
         rows[m.group(1).strip()] = dict(zip(cols, map(int, m.group(2).split())))
-    for fam in ("gemm_bf16_kernel<", "fa_tcgen05_kernel<", "align_fused_kernel"):
+    for fam in ("gemm_bf16_kernel<", "fa_wgmma_kernel<", "align_fused_kernel"):
         fam_rows = {k: v for k, v in rows.items() if k.startswith(fam)}
         assert fam_rows, fam
         for k, v in fam_rows.items():
-            assert v["UTCHMMA"] + v["UTCHMMA.2CTA"] > 0 and v["UTMALDG"] > 0 and v["LDTM"] > 0 and v["HMMA"] == 0, (k, v)
-    # cta_group::2 pair instantiations exist (last template argument true) and use the 2-CTA MMA only
-    pairs = {k: v for k, v in rows.items() if k.startswith("gemm_bf16_kernel<") and k.rstrip(">").endswith(", true")}
-    assert pairs and all(v["UTCHMMA.2CTA"] > 0 and v["UTCHMMA"] == 0 for v in pairs.values()), pairs
+            assert v["HGMMA"] > 0 and v["UTMALDG"] > 0 and v["SYNCS"] > 0 and v["HMMA"] == 0, (k, v)
     assert {k for k, v in rows.items() if v["HMMA"]} <= {k for k in rows if k.startswith("flash_attn_kernel<")}
     assert all(v["LOCAL"] == 0 for v in rows.values()), {k: v["LOCAL"] for k, v in rows.items() if v["LOCAL"]}

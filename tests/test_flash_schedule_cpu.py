@@ -1,12 +1,12 @@
-"""CPU tier: the tile walk of the tcgen05 flash-attention kernel (csrc/attn_tcgen05.cu), restated on CPU tensors.
+"""CPU tier: the tile walk of the wgmma flash-attention kernel (csrc/attn_wgmma.cu), restated on CPU tensors.
 
 What is checked without a GPU is the ALGORITHM the kernel's roles agree on, not the kernel (the GPU tier does that):
   * 128-query tiles, 64-key tiles; causal query tiles are aligned to the END of the sequence, so the ragged tile sits at the
     start (rows before 0 are zero fill, never stored) and sees one key tile: T = 528 walks 25 key tiles per head, not 29;
   * key validity = Tk bound & key-padding mask, causal limit per row: key j visible to query i iff j <= i + Tk - Tq;
-  * LAZY RESCALE: the TMEM accumulator and the row sum are expressed in a reference max that is only advanced when the
-    running max grows by more than 2^8 (kFaTau = 8 in the log2 domain); P and l use that same reference, so O / l is exact
-    whatever the policy — probabilities may exceed 1 (up to 2^8) in between;
+  * RESCALE POLICY: the accumulator and the row sum are expressed in a reference max; the kernel advances it whenever the
+    running max grows (tau = 0).  A lazy policy that advances it only when the max grows by more than 2^tau gives the same
+    O / l, because P and l use that same reference — probabilities may exceed 1 (up to 2^tau) in between;
   * rows with every key masked produce zeros (DESIGN.md "unspecified rows"; the reference attends uniformly there and
     nothing downstream reads those rows).
 The restatement is test infrastructure; no product code routes through it.
@@ -16,7 +16,7 @@ import math
 import pytest
 import torch
 
-MQ, KT, TAU = 128, 64, 8.0  # kFaMQ, KT, kFaTau of csrc/attn_tcgen05.cu
+MQ, KT, TAU = 128, 64, 0.0  # kFaMQ, kFaKT of csrc/attn_wgmma.cu; its exact running-max rescale
 
 
 def key_tiles_of(mt, Tq, Tk, causal):
@@ -124,8 +124,8 @@ def test_causal_tiles_aligned_to_the_sequence_end_walk_25_not_29_key_tiles():
 
 
 def test_lazy_rescale_policy_does_not_change_the_result():
-    """Scores that grow along the key axis force reference-max advances; tau = 0 (rescale on every growth) and tau = 8
-    (the kernel) must agree: O and l are expressed in the same reference."""
+    """Scores that grow along the key axis force reference-max advances; tau = 0 (rescale on every growth: the kernel) and
+    tau = 8 (lazy) must agree: O and l are expressed in the same reference."""
     g = torch.Generator().manual_seed(11)
     T, hd = 384, 64
     q = torch.randn(T, hd, generator=g, dtype=torch.float64)
@@ -134,7 +134,7 @@ def test_lazy_rescale_policy_does_not_change_the_result():
     sc = hd ** -0.5
     ref = reference(q, k, v, sc, False, None)
     eager, _, n_eager = flash_walk(q, k, v, sc, tau=0.0)
-    lazy, _, n_lazy = flash_walk(q, k, v, sc, tau=TAU)
+    lazy, _, n_lazy = flash_walk(q, k, v, sc, tau=8.0)
     print(f"[lazy rescale] row rescales: tau=0 {n_eager}, tau=8 {n_lazy}")
     assert 0 < n_lazy < n_eager // 2  # the threshold really skips rescales, and this input really needs some
     assert float((eager - ref).abs().max()) < 1e-10 and float((lazy - ref).abs().max()) < 1e-10

@@ -1,6 +1,6 @@
-"""CPU tier: the host side of mm_gemm_fwd (tile width from the cost model, CTA pairs / cta_group::2, rasterisation group,
-stream-K tail, argument checks) through mm_gemm_plan — the same dispatcher run without a launch.  No GPU involved: the
-library assumes 148 SMs when no device is visible.  The decisions asserted here are the ones DESIGN.md §3 / §6 document."""
+"""CPU tier: the host side of mm_gemm_fwd (tile width from the cost model, rasterisation group, stream-K tail, argument
+checks) through mm_gemm_plan — the same dispatcher run without a launch.  No GPU involved: the library assumes the 132
+SMs of an H100 SXM when no device is visible.  The decisions asserted here are the ones DESIGN.md §3 / §6 document."""
 import ctypes as C
 import random
 
@@ -9,65 +9,62 @@ import pytest
 from macaw_llm_b200 import _lib, ops
 
 E, I, V = 4096, 11008, 32000
-SMS = 148
+SMS = 132
 
 
 def plan(**kw):
     return ops.gemm_plan(**kw)
 
 
-def test_llama_gemms_at_batch_32_run_as_cta_group2_pairs():
-    M = 32 * 528
+def test_llama_gemms_at_batch_32_use_full_width_tiles():
+    M = 32 * 528  # 132 M tiles: every N column of tiles is exactly one wave
     for N, K, epi in ((3 * E, E, ops.EPI_ROPE), (E, E, ops.EPI_STD), (2 * I, E, ops.EPI_SWIGLU), (E, I, ops.EPI_STD),
                       (V, E, ops.EPI_STD)):
         p = plan(M=M, N=N, K=K, epi=epi, fp16=True, streamk=True)
-        assert (p["block_n"], p["pairs"], p["grid"], p["workers"]) == (256, 2, SMS, SMS // 2), (N, K, p)
-        assert p["units"] == (M // 256) * ((N + 255) // 256) and p["streamk_tiles"] == 0  # stream-K never rides pairs
+        assert (p["block_n"], p["pairs"], p["grid"], p["workers"]) == (128, 0, SMS, SMS), (N, K, p)
+        assert p["units"] == (M // 128) * ((N + 127) // 128) and p["waves"] == (N + 127) // 128 and p["streamk_tiles"] == 0
         assert p["smem_bytes"] <= 227 * 1024 and p["vectorised_epilogue"] == 1
-    # rasterisation group ~ 32 MiB of A rows: 16 pairs at K = 4096, 6 at K = 11008
+    # rasterisation group ~ 16 MiB of A rows: 16 M tiles at K = 4096, 6 at K = 11008
     assert plan(M=M, N=E, K=E)["group_m"] == 16 and plan(M=M, N=E, K=I)["group_m"] == 6
 
 
 def test_short_k_gemms_stay_single_cta():
-    # CLIP / Whisper layers (K = 1024 / 512): 8 - 16 k-blocks do not amortise a pair's fill (measured slower, DESIGN §6)
+    # CLIP / Whisper layers (K = 1024 / 512)
     for M, N, K in ((8224, 3072, 1024), (8224, 4096, 1024), (48000, 1536, 512), (48000, 2048, 512)):
         p = plan(M=M, N=N, K=K, fp16=True)
-        assert p["pairs"] == 0 and p["workers"] == SMS and p["grid"] == SMS, p
-    assert plan(M=8224, N=1024, K=4096, fp16=True)["pairs"] == 2  # fc2: K = 4096 -> pairs
+        assert p["pairs"] == 0 and p["workers"] == SMS and p["grid"] == SMS and p["block_n"] == 128, p
+    p = plan(M=8224, N=1024, K=4096, fp16=True)  # fc2: 65 x 8 = 520 tiles of 128 x 128 fill 4 waves (528 slots)
+    assert (p["block_n"], p["units"], p["waves"]) == (128, 520, 4)
 
 
-def test_per_gpu_batch_of_the_8_gpu_run_odd_m_tiles():
-    """M = 2112 = 17 M tiles: pairs only where the pair schedule needs no more waves than the single-CTA one."""
+def test_per_gpu_batch_of_the_8_gpu_run():
+    """M = 2112 = 17 M tiles: the tile width that needs the fewest cost-weighted waves, stream-K where the tail pays."""
     M = 4 * 528
     qkv = plan(M=M, N=3 * E, K=E, epi=ops.EPI_ROPE, fp16=True, streamk=True)
-    assert (qkv["pairs"], qkv["units"], qkv["waves"]) == (2, 9 * 48, 6)         # 816 single tiles would also be 6 waves
+    assert (qkv["block_n"], qkv["units"], qkv["waves"], qkv["streamk_tiles"]) == (128, 17 * 96, 13, 0)  # 48-tile tail: too small a saving
     gu = plan(M=M, N=2 * I, K=E, epi=ops.EPI_SWIGLU, fp16=True, streamk=True)
-    assert (gu["pairs"], gu["units"], gu["waves"]) == (0, 17 * 86, 10)          # pairs would need 11 waves
+    assert (gu["units"], gu["waves"], gu["streamk_tiles"], gu["grid"]) == (17 * 172, 23, (17 * 172) % SMS, SMS)
+    o = plan(M=M, N=E, K=E, fp16=True, streamk=True)  # 64-wide tiles: 9 waves of 128 x 64 beat 5 of 128 x 128
+    assert (o["block_n"], o["units"], o["waves"]) == (64, 17 * 64, 9)
     head = plan(M=M, N=V, K=E, fp16=True, streamk=True)
-    assert head["pairs"] == 0 and head["streamk_tiles"] == (17 * 125) % SMS == 53 and head["grid"] == SMS
-    assert plan(M=M, N=V, K=E, fp16=True, streamk=False)["streamk_tiles"] == 0  # opt-in per launch through the workspace
+    assert (head["block_n"], head["units"], head["waves"], head["grid"]) == (128, 17 * 250, 33, SMS)
+    assert plan(M=M, N=2 * I, K=E, epi=ops.EPI_SWIGLU, fp16=True, streamk=False)["streamk_tiles"] == 0  # opt-in per launch
 
 
 def test_policy_switches():
     lib = _lib.load()
-    M = 32 * 528
-    prev = lib.mm_gemm_cg2_mode(0)
-    try:
-        assert plan(M=M, N=E, K=E)["pairs"] == 1  # round 1's scheme: multicast pairs of cta_group::1 MMAs
-    finally:
-        lib.mm_gemm_cg2_mode(prev)
-    assert plan(M=M, N=E, K=E)["pairs"] == 2
     prev = lib.mm_gemm_streamk_mode(0)
     try:
-        assert plan(M=4 * 528, N=V, K=E, streamk=True)["streamk_tiles"] == 0
+        assert plan(M=4 * 528, N=2 * I, K=E, epi=ops.EPI_SWIGLU, streamk=True)["streamk_tiles"] == 0
     finally:
         lib.mm_gemm_streamk_mode(prev)
+    assert plan(M=4 * 528, N=2 * I, K=E, epi=ops.EPI_SWIGLU, streamk=True)["streamk_tiles"] == 20
     prev = lib.mm_gemm_streamk_mode(2)  # whenever the schedule allows
     try:
         p = plan(M=4 * 528, N=E, K=E, streamk=True)
-        assert p["pairs"] == 2 and p["streamk_tiles"] == 0  # ... which excludes pair launches
-        assert plan(M=1028, N=4096, K=1024, streamk=True)["streamk_tiles"] == 0   # needs more than one full wave
-        assert plan(M=8224, N=3072, K=1024, streamk=True)["streamk_tiles"] == 780 % SMS
+        assert p["streamk_tiles"] == p["units"] % SMS == 32
+        assert plan(M=1028, N=1024, K=1024, streamk=True)["streamk_tiles"] == 0   # needs more than one full wave
+        assert plan(M=8224, N=3072, K=1024, streamk=True)["streamk_tiles"] == 1560 % SMS
     finally:
         lib.mm_gemm_streamk_mode(prev)
 
@@ -94,16 +91,13 @@ def test_schedule_invariants_random_shapes():
         if b_mn:
             N = (N + 7) // 8 * 8
         p = plan(M=M, N=N, K=K, batch=batch, b_mn_major=b_mn, a_mn_major=a_mn, streamk=rng.random() < 0.5)
-        assert p["block_n"] in (32, 64, 128, 256) and (not b_mn or p["block_n"] >= 64)
+        assert p["block_n"] in (32, 64, 128) and (not b_mn or p["block_n"] >= 64)
         assert p["m_tiles"] == (M + 127) // 128 and p["n_tiles"] == (N + p["block_n"] - 1) // p["block_n"]
         assert p["k_blocks"] == (K + 63) // 64
-        m_units = (p["m_tiles"] + 1) // 2 if p["pairs"] else p["m_tiles"]
-        assert p["units"] == batch * m_units * p["n_tiles"]
-        assert p["workers"] == (SMS // 2 if p["pairs"] else SMS)
+        assert p["units"] == batch * p["m_tiles"] * p["n_tiles"] and p["pairs"] == 0
+        assert p["workers"] == SMS
         assert p["waves"] == -(-p["units"] // p["workers"]) and 0 < p["grid"] <= SMS
-        assert p["grid"] % 2 == 0 or not p["pairs"]
-        assert not (p["pairs"] and (p["block_n"] != 256 or p["k_blocks"] < 32 or a_mn))
-        assert 0 <= p["streamk_tiles"] < SMS and not (p["streamk_tiles"] and p["pairs"])
+        assert 0 <= p["streamk_tiles"] < SMS
         assert p["smem_bytes"] <= 227 * 1024 and p["group_m"] >= 2
 
 
@@ -121,7 +115,7 @@ def test_argument_checks_raise_with_a_message():
 
     assert rc()[0] == 0
     r, msg = rc(a_fp16=1, b_fp16=0)
-    assert r != 0 and "mixed f16 x bf16" in msg  # sm_100a faults on a mixed-format tcgen05.mma (measured)
+    assert r != 0 and "mixed f16 x bf16" in msg  # wgmma takes one input type for both operands
     r, msg = rc(lda=250)
     assert r != 0 and "multiples of 8" in msg
     r, msg = rc(A=fake + 2)

@@ -1,4 +1,4 @@
-"""Per-kernel numerics on the B200: every C-ABI kernel against a plain torch fp32 restatement of the same op
+"""Per-kernel numerics on the H100: every C-ABI kernel against a plain torch fp32 restatement of the same op
 (bf16-rounded inputs, fp32 math).  Tolerances are norm-wise relative errors; bf16 output rounding alone is ~2e-3
 element-wise / ~1.5e-3 norm-wise, so GEMM-class outputs are held to 4e-3 and fp32 outputs to 1e-4."""
 import math
@@ -23,7 +23,7 @@ def rel_err(a: torch.Tensor, b: torch.Tensor) -> float:
 
 
 def test_attention_lazy_rescale_large_scores():
-    """Scores with a large dynamic range (row max grows by >> 2^8 between key tiles) exercise the TMEM rescale path."""
+    """Scores with a large dynamic range (row max grows by >> 2^8 between key tiles) exercise the running-max rescale."""
     ops = _ops()
     B, H, T, hd = 1, 2, 512, 128
     q = rnd(B, T, H, hd, scale=2.0, seed=60)
@@ -214,7 +214,7 @@ def _attn_ref(q, k, v, scale, causal, key_mask):
         (2, 4, 130, 130, 128, True, True),     # LLaMA causal + right padding
         (1, 2, 64, 64, 128, True, False),
         (1, 2, 1, 70, 64, False, False),
-        (2, 32, 528, 528, 128, True, True),    # cfg4 LLaMA shape: 5 query tiles, lazy-rescale path, padding
+        (2, 32, 528, 528, 128, True, True),    # cfg4 LLaMA shape: 5 query tiles (ragged first tile), padding
         (1, 3, 300, 300, 64, True, False),
     ],
 )
@@ -330,51 +330,48 @@ def test_rms_rstd_and_fused_norm_linear():
 @pytest.mark.parametrize(
     "M,N,K,kind",
     [
-        (4224, 4096, 512, "std"),      # 33 M tiles (odd): last pair has an idle half
+        (4224, 4096, 512, "std"),      # 33 M tiles
         (4096, 2560, 1024, "bias_res"),
         (4096, 4096, 1024, "rope"),
         (4096, 5504, 1024, "swiglu"),
         (3072, 4096, 3001, "mn"),      # P x table shape, MN-major B, ragged K
         (16896, 4096, 4096, "std"),    # cfg4 o_proj
-        (2176, 12288, 4096, "rope"),   # 17 M tiles (odd): pairs only as cta_group::2 units (same wave count as single CTAs)
+        (2176, 12288, 4096, "rope"),   # 17 M tiles: a partial last wave
         (2112, 4096, 11008, "bias_res"),
     ],
 )
-@pytest.mark.parametrize("cg2", [0, 1], ids=["mc_pairs", "cta_group2"])
-def test_gemm_multicast_pairs(M, N, K, kind, cg2):
-    """Shapes large enough to take the 2-CTA path (BN = 256, >= 2 waves): as two cta_group::1 MMAs sharing a multicast B
-    tile, and as ONE cta_group::2 MMA unit (mm_gemm_cg2_mode)."""
-    from macaw_llm_b200 import _lib
-
-    prev = _lib.load().mm_gemm_cg2_mode(cg2)
-    try:
-        _multicast_pairs_case(M, N, K, kind)
-        torch.cuda.synchronize()
-    finally:
-        _lib.load().mm_gemm_cg2_mode(prev)
-
-
-def _multicast_pairs_case(M, N, K, kind):
+@pytest.mark.parametrize("dtype", ["bf16", "fp16"])
+def test_gemm_wide_shapes(M, N, K, kind, dtype):
+    """The wide, multi-wave GEMMs of the LLaMA stack and the alignment chain, with bf16 and with fp16 operands /
+    activations."""
     ops = _ops()
-    x = rnd(M, K, seed=80)
+    dt = torch.float16 if dtype == "fp16" else torch.bfloat16
+    ops.set_act_format(dt)
+    _wide_case(M, N, K, kind, dt)
+    torch.cuda.synchronize()
+
+
+def _wide_case(M, N, K, kind, dt):
+    ops = _ops()
+    x = rnd(M, K, seed=80).to(dt)
     if kind == "mn":
-        P = rnd(M, 3008, seed=81).abs()
+        P = rnd(M, 3008, seed=81).abs().to(dt)
         P[:, K:] = 0
-        tab = rnd(K, N, seed=82)
-        out = torch.empty(M, N, device=DEV, dtype=torch.bfloat16)
+        tab = rnd(K, N, seed=82).to(dt)
+        out = torch.empty(M, N, device=DEV, dtype=dt)
         ops.gemm_raw(M=M, N=N, K=K, A=P.data_ptr(), lda=P.stride(0), B=tab.data_ptr(), ldb=N, b_mn_major=True,
                      Cout=out.data_ptr(), ldc=N)
         assert rel_err(out, P[:, :K].float() @ tab.float()) < 4e-3
         return
     if kind == "swiglu":
         I = N // 2
-        wg, wu = rnd(I, K, scale=K ** -0.5, seed=83), rnd(I, K, scale=K ** -0.5, seed=84)
+        wg, wu = rnd(I, K, scale=K ** -0.5, seed=83).to(dt), rnd(I, K, scale=K ** -0.5, seed=84).to(dt)
         wgu = torch.stack([wg.view(I // 32, 32, K), wu.view(I // 32, 32, K)], dim=1).reshape(2 * I, K).contiguous()
         out = ops.linear(x, wgu, epi=ops.EPI_SWIGLU)
         ref = torch.nn.functional.silu(x.float() @ wg.float().t()) * (x.float() @ wu.float().t())
         assert rel_err(out, ref) < 4e-3
         return
-    w = rnd(N, K, scale=K ** -0.5, seed=85)
+    w = rnd(N, K, scale=K ** -0.5, seed=85).to(dt)
     if kind == "rope":
         T = 128
         inv = 1.0 / (10000 ** (torch.arange(0, 128, 2, device=DEV).float() / 128))
@@ -388,7 +385,7 @@ def _multicast_pairs_case(M, N, K, kind):
         assert rel_err(out, ref) < 4e-3
         return
     if kind == "bias_res":
-        b, res = rnd(N, seed=86), rnd(M, N, seed=87)
+        b, res = rnd(N, seed=86).to(dt), rnd(M, N, seed=87).to(dt)
         out = ops.linear(x, w, b, residual=res)
         assert rel_err(out, x.float() @ w.float().t() + b.float() + res.float()) < 4e-3
         return
@@ -397,13 +394,15 @@ def _multicast_pairs_case(M, N, K, kind):
 
 
 @pytest.mark.parametrize("M,N,K,kind", [
-    (2112, 4096, 4096, "res_stats"),   # o_proj at 4 samples/GPU: 272 tiles -> 1 wave + 124 (every CTA: finisher + contributor)
+    (2112, 4096, 4096, "res_stats"),   # o_proj at 4 samples/GPU: 17 x 64 = 1088 tiles of 128 x 64 -> 8 waves + 32
     (2112, 4096, 11008, "res_stats"),  # down_proj, K = 172 k-blocks
-    (2112, 12288, 4096, "rope"),       # QKV + RoPE: 816 tiles -> 5 waves + 76
-    (1200, 4096 * 2, 1024, "swiglu"),  # 10 x 32 = 320 tiles -> 2 waves + 24: shares of ~3 k-blocks, 6+ contributors per tile
-                                       # (K = 1024 keeps the launch off the multicast-pair path, which has no stream-K)
-    (19072, 256, 4096, "plain"),       # 149 tiles -> 1 wave + 1: ONE tile split over 64 CTAs (63 contributors)
-    (640, 7680, 512, "plain"),         # 5 x 30 = 150 tiles, num_k = 8: shares shorter than one k-block for most CTAs
+    (2112, 12288, 4096, "rope"),       # QKV + RoPE: 17 x 96 = 1632 tiles -> 12 waves + 48
+    (264, 12288, 4096, "rope"),        # cfg2 QKV + RoPE (B=1, T=264): 3 x 96 = 288 tiles -> 2 waves + 24; each RoPE
+                                       # warp owns columns (i, i + 64) of a head: its partials must come from that warp
+    (1200, 4096 * 2, 1024, "swiglu"),  # 10 x 64 = 640 tiles -> 4 waves + 112: shares of ~14 of a tile's 16 k-blocks
+    (19072, 256, 4096, "plain"),       # 149 x 4 = 596 tiles of 128 x 64 -> 4 waves + 68: a narrow N, long K
+    (17024, 64, 4096, "plain"),        # 133 tiles -> 1 wave + 1: ONE tile split over all CTAs (64 k-blocks on 132 CTAs)
+    (640, 7680, 512, "plain"),         # 5 x 120 = 600 tiles, num_k = 8: shares shorter than one k-block for most CTAs
 ])
 def test_gemm_streamk_tail(M, N, K, kind):
     """Stream-K tail (mm_gemm_args.sk_workspace): the partial last wave's k-blocks are split evenly over all CTAs, partial
@@ -429,18 +428,14 @@ def test_gemm_streamk_tail(M, N, K, kind):
     cos_g, sin_g = torch.rand(528, 64, device=DEV), torch.rand(528, 64, device=DEV)
     from macaw_llm_b200 import _lib
 
-    prev_cg2 = _lib.load().mm_gemm_cg2_mode(0)  # M = 2112 would otherwise run as cta_group::2 pairs (no stream-K there)
+    base, base_ss = run()
+    ops.STREAMK = ws
+    prev = _lib.load().mm_gemm_streamk_mode(2)  # force: the default policy skips shapes where it does not pay (o_proj)
     try:
-        base, base_ss = run()
-        ops.STREAMK = ws
-        prev = _lib.load().mm_gemm_streamk_mode(2)  # force: the default policy skips shapes where it does not pay (o_proj)
-        try:
-            outs = [run() for _ in range(3)]
-        finally:
-            ops.STREAMK = None
-            _lib.load().mm_gemm_streamk_mode(prev)
+        outs = [run() for _ in range(3)]
     finally:
-        _lib.load().mm_gemm_cg2_mode(prev_cg2)
+        ops.STREAMK = None
+        _lib.load().mm_gemm_streamk_mode(prev)
     torch.cuda.synchronize()
     assert int(ws[:2048].abs().sum()) == 0  # every flag re-armed
     got, got_ss = outs[0]
@@ -595,9 +590,9 @@ def test_rope_rows_and_swiglu_rows():
 
 # ------------------------------------------------------------------------------------------------ fp16 activation chain
 def test_gemm_fp16_operands():
-    """tcgen05 kind::f16 with fp16 A and B operands and fp16 output: the alignment chain's format.  One fp16 rounding is
-    ~1.4e-4 norm-wise (bf16: ~1.1e-3).  Mixed f16 x bf16 is rejected up front: sm_100a raises an illegal-instruction
-    fault for it even though the instruction descriptor has independent format fields (measured in round 2)."""
+    """wgmma .f16 with fp16 A and B operands and fp16 output: the alignment chain's format.  One fp16 rounding is
+    ~1.4e-4 norm-wise (bf16: ~1.1e-3).  Mixed f16 x bf16 is rejected up front: wgmma takes one input type for both
+    operands."""
     ops = _ops()
     M, N, K = 200, 768, 1096
     g = torch.Generator().manual_seed(5)

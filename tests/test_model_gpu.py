@@ -1,4 +1,4 @@
-"""End-to-end parity of the CUDA path on the B200 against (a) the golden vectors minted from the unmodified reference
+"""End-to-end parity of the CUDA path on the H100 against (a) the golden vectors minted from the unmodified reference
 and (b) the CPU oracle run on the SAME bf16-rounded weights and inputs.
 
 Tolerances (norm-wise relative error, ||ours - ref|| / ||ref||):

@@ -1,5 +1,5 @@
-"""CPU tier: the oracle (oracle/macaw_oracle.py) against the golden vectors minted from the unmodified reference, and
-— when /root/reference exists (build container) — against the live reference in-process."""
+"""CPU tier: the oracle (oracle/macaw_oracle.py) against the golden vectors minted from the unmodified reference
+(tests/golden/make_golden.py runs the reference in-process and stores what it computed)."""
 import os
 
 import numpy as np
@@ -155,16 +155,12 @@ def test_philox_known_answers():
     assert abs(float((m != 0).mean()) - 0.9) < 0.03
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference"), reason="reference tree only exists in the build container")
-def test_oracle_vs_live_reference():
-    from tests.golden import make_golden as MG
-
-    modeling = MG.import_reference()
-    cfg, model, shapes, weights = MG.build_reference(modeling, gen.TINY)
-    hp = O.hp_from_config(cfg)
+def test_oracle_vs_live_reference(tiny_weights):
+    """The reference module's own fp32 forward on one seeded batch (tests/golden/tiny_live_ref.npz, written by
+    make_golden.live_reference_fixtures) against the oracle on the same weights."""
+    spec, hp, weights = tiny_weights
+    ref = np.load(os.path.join(H.GOLDEN, "tiny_live_ref.npz"))
     inp = gen.make_inputs(gen.TINY, 2, 11, seed=7, modalities=("image", "audio"), pad_tail=2)
-    with torch.no_grad():
-        out = model(inp)
-    o = O.forward(inp, {k: v for k, v in model.state_dict().items()}, hp)
-    assert H.rel_err(o["logits"], out.logits) < 1e-4
-    assert abs(float(o["loss"]) - float(out.loss)) < 1e-4
+    o = O.forward(inp, weights, hp)
+    assert H.rel_err(o["logits"], torch.from_numpy(ref["logits"])) < 1e-4
+    assert abs(float(o["loss"]) - float(ref["loss"])) < 1e-4

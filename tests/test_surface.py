@@ -198,3 +198,29 @@ def test_grad_buffer_layout_and_reference_freezing():
     assert not again[id(llm.lm_head.weight)] and again[id(model.video_align_attention.in_proj_weight)]
     gb.zero()
     assert llm.lm_head.weight.grad is None
+
+
+def test_grad_buffer_with_frozen_decoder_layers():
+    """freeze_llama_layers (bench.py --mode train): frozen decoder layers leave the trainable set and the flat gradient
+    buffer (their bucket is empty, so no optimizer state either); every other parameter keeps its slot and order."""
+    from macaw_llm_b200.training import GradBuffer, freeze_like_reference, freeze_llama_layers, trainable_parameters
+
+    model, spec, hp, _ = H.build_tiny_model("cpu", torch.bfloat16)
+    freeze_like_reference(model)
+    full = GradBuffer(model)
+    freeze_llama_layers(model, 1)
+    frozen = {n for n, p in model.named_parameters() if n.startswith("llm.model.layers.0.")}
+    assert frozen and all(not p.requires_grad for n, p in model.named_parameters() if n in frozen)
+    assert all(p.requires_grad for n, p in model.named_parameters() if n.startswith("llm.model.layers.1."))
+    train = dict(trainable_parameters(model))
+    assert not (set(train) & frozen)
+    gb = GradBuffer(model)
+    assert {id(p) for p in gb.params} == {id(p) for p in train.values()}
+    L = len(model.llm.model.layers)
+    assert len(gb.buckets) == L + 2 and gb.buckets[L][0] == gb.buckets[L][1]  # layer 0 = the last layer bucket: empty
+    n_frozen = sum(p.numel() for n, p in model.named_parameters() if n in frozen)
+    assert gb.flat.numel() == full.flat.numel() - n_frozen
+    with pytest.raises(ValueError):
+        freeze_llama_layers(model, L + 1)
+    freeze_llama_layers(model, 0)
+    assert all(p.requires_grad for p in model.llm.parameters())

@@ -1,4 +1,4 @@
-"""Training step on the B200 (SURVEY.md §8f rank 1): every backward kernel against torch autograd of the same op, the
+"""Training step on the H100 (SURVEY.md §8f rank 1): every backward kernel against torch autograd of the same op, the
 whole decoder's gradients against autograd of the CPU oracle (fp32, same bf16-rounded weights), the fused AdamW against
 torch.optim.AdamW, and a few optimisation steps through the public `model(inputs).loss.backward()` path.
 
@@ -313,3 +313,54 @@ def test_gradient_accumulation_and_optimizer_steps(tiny_train):
         ev = float(model(inp).loss)
     print(f"\n[train loop] losses {['%.4f' % l for l in losses]}  eval after {ev:.4f}")
     assert losses[-1] < losses[0] - 0.05 and ev < losses[0]
+
+
+def test_frozen_decoder_layers_get_no_gradient(tiny_train):
+    """The lower decoder layers frozen (as bench.py --mode train does to fit one 80 GB GPU): they get no gradient and no
+    optimizer update, the backward pass still runs through them, so every other gradient — the alignment modules' and the
+    table's included — is the one the fully trainable step computes."""
+    from macaw_llm_b200.training import FusedAdamW, freeze_llama_layers, trainable_parameters
+    from tests.golden import gen
+    import copy
+
+    model0, spec, hp, weights = tiny_train
+    inp = gen.make_inputs(spec, 2, 16, seed=9, modalities=("image", "audio"), with_labels=True)
+    inp = {k: (v.to(torch.bfloat16).cuda() if isinstance(v, torch.Tensor) and v.is_floating_point() else
+               (v.cuda() if isinstance(v, torch.Tensor) else v)) for k, v in inp.items()}
+
+    def grads(m):
+        m.train()
+        m.train_step.attention_dropout = False
+        try:
+            for p in m.parameters():
+                p.grad = None
+            m(inp).loss.backward()
+            torch.cuda.synchronize()
+        finally:
+            m.train_step.attention_dropout = True
+            m.eval()
+        return {n: (p.grad.float().clone() if p.grad is not None else None) for n, p in m.named_parameters()}
+
+    full = grads(copy.deepcopy(model0))
+    model = copy.deepcopy(model0)
+    freeze_llama_layers(model, 1)
+    part = grads(model)
+    frozen = {n for n, _ in model.named_parameters() if n.startswith("llm.model.layers.0.")}
+    assert frozen and not ({n for n, _ in trainable_parameters(model)} & frozen)
+    for n, g in full.items():
+        if n in frozen:
+            assert part[n] is None, n
+        elif g is not None:
+            assert part[n] is not None and rel(part[n], g) < 2e-3, n  # bf16 atomics in the table scatter may reorder sums
+    w0 = model.llm.model.layers[0].mlp.down_proj.weight.detach().clone()
+    w1 = model.llm.model.layers[1].mlp.down_proj.weight.detach().clone()
+    opt = FusedAdamW([p for _, p in trainable_parameters(model)], lr=1e-3, weight_decay=0.0)
+    model.train()
+    try:
+        model(inp).loss.backward()
+        opt.step()
+        torch.cuda.synchronize()
+    finally:
+        model.eval()
+    assert torch.equal(model.llm.model.layers[0].mlp.down_proj.weight, w0)
+    assert not torch.equal(model.llm.model.layers[1].mlp.down_proj.weight, w1)

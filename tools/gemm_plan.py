@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """Schedules the GEMM dispatcher picks for the dense GEMMs of the BASELINE configs at every per-GPU batch of the 1/2/4/8-GPU
-run (mm_gemm_plan: the host side of mm_gemm_fwd without a launch — no GPU needed, the library assumes 148 SMs).
+run (mm_gemm_plan: the host side of mm_gemm_fwd without a launch — no GPU needed, the library assumes the 132 SMs of an H100 SXM).
 
 Explains the strong-scaling curve from the schedule alone: `fill` = share of the scheduled tile slots that carry work
-(wave quantisation + the idle half of an odd last pair), next to the padded-row share of the last M tile.
-Usage: python tools/gemm_plan.py > profiles/r2_gemm_schedules.txt
+(wave quantisation), next to the padded-row share of the last M tile.
+Usage: python tools/gemm_plan.py
 """
 import os
 import sys
@@ -14,15 +14,12 @@ sys.path.insert(0, ROOT)
 
 from macaw_llm_b200 import ops  # noqa: E402
 
-PAIRS = {0: "single", 1: "mc-pair", 2: "cg2-pair"}
-
-
 def row(name, M, N, K, **kw):
     p = ops.gemm_plan(M=M, N=N, K=K, **kw)
     pad = 1.0 - M / (p["m_tiles"] * 128.0)
     eff = p["fill"] * (1.0 - pad) if p["streamk_tiles"] == 0 else (1.0 - pad)  # stream-K shares the tail over all CTAs
     flops = 2.0 * M * N * K
-    return (f"  {name:22s} M={M:6d} N={N:6d} K={K:6d}  BN={p['block_n']:3d} {PAIRS[p['pairs']]:8s} units={p['units']:5d} "
+    return (f"  {name:22s} M={M:6d} N={N:6d} K={K:6d}  BN={p['block_n']:3d} units={p['units']:5d} "
             f"waves={p['waves']:3d} fill={p['fill']:.3f} pad={pad:.3f} group_m={p['group_m']:2d} streamk_tiles={p['streamk_tiles']:3d} "
             f"-> useful share of the scheduled MMA slots {eff:.3f}"), flops, eff
 
@@ -41,7 +38,7 @@ def family(title, rows):
 
 def main():
     E, I, V = 4096, 11008, 32000
-    print("# tools/gemm_plan.py — schedules from mm_gemm_plan (host-side dispatch of mm_gemm_fwd, 148 SMs, fp16 operands)")
+    print("# tools/gemm_plan.py — schedules from mm_gemm_plan (host-side dispatch of mm_gemm_fwd, 132 SMs, fp16 operands)")
     print("# fill = units / (waves x workers); pad = padded rows of the last 128-row M tile; stream-K launches count the tail as")
     print("# fully shared.  cfg4: T = 528 positions per sample, 257 CLIP tokens per image, 1500 Whisper frames per clip.")
     for B in (32, 16, 8, 4):

@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """SASS / resource inventory of libmacaw_b200.so (no GPU needed: `cuobjdump` reads the cubin nvcc cross-compiled).
 
-Per kernel: registers, static + dynamic-independent shared memory, local (spill) bytes, and how often the Blackwell
-mnemonics that prove a tcgen05 / TMEM / TMA kernel appear (UTCHMMA = tcgen05.mma, `.2CTA` = cta_group::2, UTMALDG = TMA
-tensor load, `.MULTICAST` = cluster multicast, LDTM / STTM = tcgen05.ld / st, UTCBAR = tcgen05.commit) next to the
-pre-Blackwell HMMA (mma.sync).  Usage: python tools/sass_inventory.py > profiles/r2_sass_inventory.txt
+Per kernel: registers, static + dynamic-independent shared memory, local (spill) bytes, and how often the Hopper
+mnemonics that prove a wgmma / TMA / mbarrier kernel appear (HGMMA = wgmma.mma_async, UTMALDG = TMA tensor load,
+SYNCS = mbarrier operations, WARPGROUP = warpgroup arrive / wait) next to HMMA (mma.sync).
+Usage: python tools/sass_inventory.py
 """
 import os
 import re
@@ -16,9 +16,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "macaw-llm_b200", "libmacaw_b200.so")
 
 COLS = OrderedDict([
-    ("UTCHMMA", r"\bUTCHMMA\b(?!\.2CTA)"), ("UTCHMMA.2CTA", r"\bUTCHMMA\.2CTA"), ("UTMALDG", r"\bUTMALDG"),
-    ("TMA.MCAST", r"\bUTMALDG\S*MULTICAST"), ("LDTM", r"\bLDTM"), ("STTM", r"\bSTTM"), ("UTCBAR", r"\bUTCBAR"),
-    ("HMMA", r"(?<!UTC)\bHMMA\."), ("MUFU.EX2", r"\bMUFU\.EX2"), ("FFMA2", r"\bFFMA2"),
+    ("HGMMA", r"\bHGMMA\."), ("UTMALDG", r"\bUTMALDG"), ("SYNCS", r"\bSYNCS\."), ("WARPGROUP", r"\bWARPGROUP\."),
+    ("HMMA", r"\bHMMA\."), ("MUFU.EX2", r"\bMUFU\.EX2"),
 ])
 
 
@@ -69,8 +68,8 @@ def main():
     arch = re.search(r"arch = (\S+)", run("cuobjdump", "-lelf", LIB) + sass)
     print(f"# tools/sass_inventory.py over macaw-llm_b200/libmacaw_b200.so ({arch.group(1) if arch else '?'}; "
           f"{len(counts)} kernels; cuobjdump -sass / --dump-resource-usage, no GPU involved)")
-    print("# UTCHMMA = tcgen05.mma (.2CTA = cta_group::2), UTMALDG = TMA tensor load (TMA.MCAST = .MULTICAST variants),")
-    print("# LDTM/STTM = tcgen05.ld/st, UTCBAR = tcgen05.commit, HMMA = mma.sync (pre-Blackwell pipe), LOCAL = spill bytes")
+    print("# HGMMA = wgmma.mma_async, UTMALDG = TMA tensor load, SYNCS = mbarrier operations, WARPGROUP = warpgroup")
+    print("# arrive / wait, HMMA = mma.sync, LOCAL = spill bytes")
     hdr = f"{'kernel':64s} {'REG':>4s} {'SMEM':>6s} {'LOCAL':>5s} " + " ".join(f"{k:>12s}" for k in COLS)
     print(hdr)
     tot = defaultdict(int)
