@@ -371,15 +371,57 @@ int32_t mm_dropout_mask(float* out, int64_t ld, int32_t rows, int32_t cols, floa
  * upstream gradient of the loss as a device scalar, so the launch is CUDA-graph capturable) / n_valid; may run in place. */
 int32_t mm_ce_bwd(const void* logits, const int64_t* labels, void* dlogits, int32_t B, int32_t T, int32_t V,
                   const int32_t* n_valid, float grad_scale, const float* grad_scale_dev, void* stream);
-/* Gradient of mm_embed_gather: dtable[ids[i], :] += dx[i, :] (bf16x2 atomics). */
+/* Gradient of mm_embed_gather: dtable[ids[i], :] += dx[i, :] (bf16x2 atomics; half2 atomics in fp16). */
 int32_t mm_embed_scatter_add(const void* dx, int64_t ldx, const int64_t* ids, int64_t n, int32_t dim, int32_t vocab,
                              void* dtable, void* stream);
 /* out[c] += sum_r x[r, c]  (bias gradients; fp32 atomics) */
 int32_t mm_colsum(const void* x, int64_t ldx, int32_t rows, int32_t cols, float* out, void* stream);
-/* Fused AdamW step on one parameter tensor: bf16 working copy p, bf16 gradient g (times grad_scale), fp32 master / m / v.
- * The bias corrections use `step`, or the device int *step_dev when given (graph-replayed training steps). */
+/* Fused AdamW step on one parameter tensor: 16-bit working copy p and gradient g in the activation format (g times
+ * grad_scale), fp32 master / m / v.  The bias corrections use `step`, or the device int *step_dev when given
+ * (graph-replayed training steps).  grad_mult_dev (nullable): a device fp32 multiplier that replaces grad_scale — the
+ * unscale-and-clip factor of mm_loss_scale_update (DeepSpeed FP16_Optimizer.unscale_and_clip_grads).  skip_dev
+ * (nullable): a device int; when non-zero the launch writes nothing (p, master, m, v unchanged: the overflow-skipped
+ * step of DeepSpeed's fp16 optimizer).  With both null the behaviour is that of ABI 3. */
 int32_t mm_adamw(void* p, const void* g, float* master, float* m, float* v, int64_t n, float lr, float beta1, float beta2,
-                 float eps, float weight_decay, int32_t step, const int32_t* step_dev, float grad_scale, void* stream);
+                 float eps, float weight_decay, int32_t step, const int32_t* step_dev, float grad_scale,
+                 const float* grad_mult_dev, const int32_t* skip_dev, void* stream);
+
+/* ------------------------------------------------------------------------------------------------ loss scaling / clipping
+ * fp16 training with dynamic loss scaling and global gradient-norm clipping, on the device and free of host syncs (the
+ * whole optimizer step stays CUDA-graph capturable).  Reference: train.sh `--fp16 True` with DeepSpeed's fp16 optimizer,
+ * configs/deepspeed_config.json "fp16" block (loss_scale 0 = dynamic, initial_scale_power 16, loss_scale_window 1000,
+ * hysteresis 2, min_loss_scale 1) and "gradient_clipping": "auto" = HF TrainingArguments.max_grad_norm (1.0).
+ *
+ * mm_grad_sumsq: *out += sum_i g[i]^2 (fp32) over a flat 16-bit gradient buffer (fp16 != 0: IEEE half, else bf16; g
+ *   16-byte aligned, 64-bit n).  Deterministic: the grid is fixed by (n, device), `partials` (mm_grad_sumsq_parts(n) fp32)
+ *   holds one partial per CTA, summed in a fixed order.  A NaN / Inf element makes the result non-finite (overflow test).
+ *   Several ranges can be summed into one scalar by successive calls (fixed order = deterministic total). */
+int32_t mm_grad_sumsq_parts(int64_t n);
+int32_t mm_grad_sumsq(const void* g, int64_t n, int32_t fp16, float* out, float* partials, void* stream);
+/* Device-side state of the loss scaler (DeepSpeed DynamicLossScaler) and of the optimizer step it gates. */
+typedef struct mm_loss_scale_state {
+  float scale;                /* S: the loss is multiplied by S before backward */
+  float inv_scale;            /* 1 / S */
+  int32_t cur_iter;           /* optimizer steps seen (skipped ones included) */
+  int32_t last_overflow_iter; /* -1 initially */
+  int32_t cur_hysteresis;     /* overflows still tolerated before the scale is halved */
+  int32_t skip;               /* 1: the latest step's gradients were non-finite; mm_adamw(skip_dev) writes nothing */
+  float grad_mult;            /* per-element gradient multiplier of the latest step: 1 / (S * max(clip, 1)) */
+  int32_t skipped;            /* skipped steps so far */
+  int32_t step;               /* AdamW step counter (bias corrections), advanced on steps that are not skipped */
+  float grad_norm;            /* unscaled global gradient norm of the latest step (non-finite on overflow) */
+  int32_t reserved[2];
+} mm_loss_scale_state;
+/* mm_loss_scale_update: one single-thread launch after the gradient sum of squares, before the AdamW launches.
+ *   overflow = !isfinite(*sumsq);  norm = sqrt(*sumsq) / S;
+ *   grad_mult = 1 / (S * max((norm + 1e-6) / max_norm, 1))  (max_norm > 0: clipping on), else 1 / S;
+ *   skip = overflow (counted in `skipped`), else step += 1;
+ *   dynamic != 0: DynamicLossScaler.update_scale — on overflow, S = max(S / 2, min_scale) if hysteresis == 1 or
+ *   cur_hysteresis == 1, else cur_hysteresis -= 1, and last_overflow_iter = cur_iter; without overflow, when
+ *   (cur_iter - last_overflow_iter) % window == 0: cur_hysteresis = hysteresis, S *= 2.  At S == min_scale an overflow
+ *   keeps S (a kernel cannot raise) and the step is skipped.  Then cur_iter += 1.  *sumsq is reset to 0. */
+int32_t mm_loss_scale_update(mm_loss_scale_state* state, float* sumsq, float max_norm, int32_t dynamic, int32_t window,
+                             int32_t hysteresis, float min_scale, void* stream);
 
 /* Backward of the absorbed alignment attention through its (V + 2)-key softmax (reference: autograd of
  * nn.MultiheadAttention, modeling.py:986-987 / 1007-1008 / 1025-1026).  See train_kernels.cu for the formulas. */
@@ -401,7 +443,8 @@ int32_t mm_cast_f16_bf16(const void* x, int64_t ldx, void* y, int64_t ldy, int32
  * reduce-scatter / all-gather, configs/deepspeed_config.json:22-41; north_star: "a single NCCL all-reduce on gradients").
  * NCCL is bound at run time (dlopen); one communicator per process (one process per GPU).  Bootstrap: rank 0 calls
  * mm_nccl_unique_id, ships the 128 bytes to the other ranks (any channel: torch.distributed store, MPI, a file), every
- * rank calls mm_nccl_init.  mm_nccl_allreduce is in place, asynchronous on `stream`; dtype 0 = bf16, 1 = fp32;
+ * rank calls mm_nccl_init.  mm_nccl_allreduce is in place, asynchronous on `stream`; dtype 0 = bf16, 1 = fp32, 2 = fp16
+ * (the gradients of an fp16 model: the loss-scale overflow test runs after the all-reduce, so every rank skips alike);
  * average != 0 divides by the group size (ncclAvg). */
 int32_t mm_nccl_unique_id(void* out128);
 int32_t mm_nccl_init(const void* id128, int32_t world, int32_t rank);

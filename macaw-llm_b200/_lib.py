@@ -77,6 +77,14 @@ class AlignArgs(C.Structure):
     ]
 
 
+class LossScaleState(C.Structure):
+    """Mirror of `mm_loss_scale_state` (include/macaw_b200.h): 12 four-byte fields."""
+
+    _fields_ = [("scale", c_f32), ("inv_scale", c_f32), ("cur_iter", c_i32), ("last_overflow_iter", c_i32),
+                ("cur_hysteresis", c_i32), ("skip", c_i32), ("grad_mult", c_f32), ("skipped", c_i32), ("step", c_i32),
+                ("grad_norm", c_f32), ("reserved", c_i32 * 2)]
+
+
 class ImageArgs(C.Structure):
     """Mirror of `mm_image_args` (include/macaw_b200.h)."""
 
@@ -135,7 +143,11 @@ SIGNATURES = {
     "mm_ce_bwd": (c_i32, [c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_vp, c_f32, c_vp, c_vp]),
     "mm_embed_scatter_add": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp]),
     "mm_colsum": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_vp]),
-    "mm_adamw": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_i32, c_vp, c_f32, c_vp]),
+    "mm_adamw": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_i32, c_vp, c_f32, c_vp,
+                         c_vp, c_vp]),
+    "mm_grad_sumsq_parts": (c_i32, [c_i64]),
+    "mm_grad_sumsq": (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp, c_vp]),
+    "mm_loss_scale_update": (c_i32, [c_vp, c_vp, c_f32, c_i32, c_i32, c_i32, c_f32, c_vp]),
     "mm_image_preprocess": (c_i32, [C.POINTER(ImageArgs), c_vp]),
     "mm_log_mel": (c_i32, [c_vp, c_i32, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_vp]),
     "mm_align_softmax_bwd": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_f32, c_vp, c_vp, c_i64, c_vp, c_i32,
@@ -151,7 +163,7 @@ SIGNATURES = {
 }
 
 _lib = None
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 
 def load(build_if_missing: bool = True) -> C.CDLL:

@@ -40,12 +40,6 @@ __device__ __forceinline__ float block_max(float v, float* sh) {
   return r;
 }
 
-// value-level 16-bit conversions in the activation format F16 (the pointers keep the `bf16` spelling: 16-bit storage)
-template <bool F16>
-__device__ __forceinline__ float ldv(bf16 v) { return cvt_in<F16>(__bfloat16_as_ushort(v)); }
-template <bool F16>
-__device__ __forceinline__ bf16 stv(float v) { return __ushort_as_bfloat16(cvt_out<F16>(v)); }
-
 __device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
   f[0] = bf16lo(u.x); f[1] = bf16hi(u.x); f[2] = bf16lo(u.y); f[3] = bf16hi(u.y);
   f[4] = bf16lo(u.z); f[5] = bf16hi(u.z); f[6] = bf16lo(u.w); f[7] = bf16hi(u.w);

@@ -95,9 +95,9 @@ extern "C" int32_t mm_nccl_init(const void* id128, int32_t world, int32_t rank) 
 extern "C" int32_t mm_nccl_allreduce(void* buf, int64_t count, int32_t dtype, int32_t average, void* stream) {
   MM_REQUIRE(buf != nullptr && count > 0, "mm_nccl_allreduce: bad arguments");
   MM_REQUIRE(g_nccl.comm != nullptr, "mm_nccl_allreduce: no communicator (mm_nccl_init was not called)");
-  // ncclDataType_t: ncclFloat32 = 7, ncclBfloat16 = 9;  ncclRedOp_t: ncclSum = 0, ncclAvg = 4
-  const int dt = dtype == 1 ? 7 : 9;
-  MM_REQUIRE(dtype == 0 || dtype == 1, "mm_nccl_allreduce: dtype must be 0 (bf16) or 1 (fp32)");
+  // ncclDataType_t: ncclFloat16 = 6, ncclFloat32 = 7, ncclBfloat16 = 9;  ncclRedOp_t: ncclSum = 0, ncclAvg = 4
+  MM_REQUIRE(dtype == 0 || dtype == 1 || dtype == 2, "mm_nccl_allreduce: dtype must be 0 (bf16), 1 (fp32) or 2 (fp16)");
+  const int dt = dtype == 1 ? 7 : (dtype == 2 ? 6 : 9);
   const int rc = g_nccl.all_reduce(buf, buf, static_cast<size_t>(count), dt, average ? 4 : 0, g_nccl.comm,
                                    reinterpret_cast<cudaStream_t>(stream));
   return nccl_check(rc, "ncclAllReduce");

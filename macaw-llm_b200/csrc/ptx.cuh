@@ -278,5 +278,10 @@ template <bool F16>
 __device__ __forceinline__ uint4 pack8t(const float (&f)[8]) {
   return make_uint4(pack2<F16>(f[0], f[1]), pack2<F16>(f[2], f[3]), pack2<F16>(f[4], f[5]), pack2<F16>(f[6], f[7]));
 }
+// value-level 16-bit conversions in the activation format F16 (the pointers keep the `bf16` spelling: 16-bit storage)
+template <bool F16>
+__device__ __forceinline__ float ldv(__nv_bfloat16 v) { return cvt_in<F16>(__bfloat16_as_ushort(v)); }
+template <bool F16>
+__device__ __forceinline__ __nv_bfloat16 stv(float v) { return __ushort_as_bfloat16(cvt_out<F16>(v)); }
 
 }  // namespace mm

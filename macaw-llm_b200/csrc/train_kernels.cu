@@ -15,13 +15,6 @@ namespace mm {
 
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
 
-__device__ __forceinline__ void unpack8f(const uint4& u, float (&f)[8]) {
-  f[0] = bf16lo(u.x); f[1] = bf16hi(u.x); f[2] = bf16lo(u.y); f[3] = bf16hi(u.y);
-  f[4] = bf16lo(u.z); f[5] = bf16hi(u.z); f[6] = bf16lo(u.w); f[7] = bf16hi(u.w);
-}
-__device__ __forceinline__ uint4 pack8f(const float (&f)[8]) {
-  return make_uint4(pack_bf16x2(f[0], f[1]), pack_bf16x2(f[2], f[3]), pack_bf16x2(f[4], f[5]), pack_bf16x2(f[6], f[7]));
-}
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -59,7 +52,7 @@ __device__ __forceinline__ float block_max(float v, float* sh) {
 constexpr int kNormMaxChunks = 4;  // cols <= 256 threads * 8 * 4 = 8192
 // NCH = 8-column chunks per thread (cols <= 256 * 8 * NCH): a template parameter so that the register budget follows the row
 // width (the fixed 4-chunk version needed 162 registers -> ONE CTA per SM at cols = 4096: 55 us per launch).
-template <int NCH>
+template <int NCH, bool F16>
 __global__ void __launch_bounds__(256) rmsnorm_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ x,
                                                           const float* __restrict__ rstd, const bf16* __restrict__ g,
                                                           const bf16* __restrict__ dres, bf16* __restrict__ dx,
@@ -74,7 +67,7 @@ __global__ void __launch_bounds__(256) rmsnorm_bwd_kernel(const bf16* __restrict
     const int c = threadIdx.x + k * blockDim.x;
 #pragma unroll
     for (int i = 0; i < 8; ++i) gacc[k][i] = 0.f;
-    if (c < nch) unpack8f(__ldg(reinterpret_cast<const uint4*>(g + c * 8)), gv[k]);
+    if (c < nch) unpack8t<F16>(__ldg(reinterpret_cast<const uint4*>(g + c * 8)), gv[k]);
   }
   const int r0 = blockIdx.x * rows_per_cta, r1 = min(rows, r0 + rows_per_cta);
   for (int r = r0; r < r1; ++r) {
@@ -93,8 +86,8 @@ __global__ void __launch_bounds__(256) rmsnorm_bwd_kernel(const bf16* __restrict
       const int c = threadIdx.x + k * blockDim.x;
       if (c < nch) {
         float dv[8];
-        unpack8f(*reinterpret_cast<const uint4*>(dy + static_cast<long long>(r) * cols + c * 8), dv);
-        unpack8f(*reinterpret_cast<const uint4*>(x + static_cast<long long>(r) * cols + c * 8), xv[k]);
+        unpack8t<F16>(*reinterpret_cast<const uint4*>(dy + static_cast<long long>(r) * cols + c * 8), dv);
+        unpack8t<F16>(*reinterpret_cast<const uint4*>(x + static_cast<long long>(r) * cols + c * 8), xv[k]);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
           tv[k][i] = dv[i] * gv[k][i];
@@ -110,10 +103,10 @@ __global__ void __launch_bounds__(256) rmsnorm_bwd_kernel(const bf16* __restrict
       const int c = threadIdx.x + k * blockDim.x;
       if (c < nch) {
         float o[8];
-        unpack8f(dru[k], o);  // zeros when there is no residual-branch gradient
+        unpack8t<F16>(dru[k], o);  // zeros when there is no residual-branch gradient
 #pragma unroll
         for (int i = 0; i < 8; ++i) o[i] += rs * tv[k][i] - coef * xv[k][i];
-        *reinterpret_cast<uint4*>(dx + static_cast<long long>(r) * cols + c * 8) = pack8f(o);
+        *reinterpret_cast<uint4*>(dx + static_cast<long long>(r) * cols + c * 8) = pack8t<F16>(o);
       }
     }
   }
@@ -168,35 +161,37 @@ __global__ void __launch_bounds__(256) dg_reduce_kernel(const float* __restrict_
 }
 
 // ------------------------------------------------------------------------------------------------ SwiGLU
+template <bool F16>
 __global__ void swiglu_fwd_kernel(const bf16* __restrict__ gate, const bf16* __restrict__ up, bf16* __restrict__ h,
                                   long long n8) {
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n8;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     float a[8], b[8], o[8];
-    unpack8f(reinterpret_cast<const uint4*>(gate)[i], a);
-    unpack8f(reinterpret_cast<const uint4*>(up)[i], b);
+    unpack8t<F16>(reinterpret_cast<const uint4*>(gate)[i], a);
+    unpack8t<F16>(reinterpret_cast<const uint4*>(up)[i], b);
 #pragma unroll
     for (int k = 0; k < 8; ++k) o[k] = a[k] / (1.f + __expf(-a[k])) * b[k];
-    reinterpret_cast<uint4*>(h)[i] = pack8f(o);
+    reinterpret_cast<uint4*>(h)[i] = pack8t<F16>(o);
   }
 }
 // dgate = dh * up * d silu(gate),  dup = dh * silu(gate);   d silu(a) = s (1 + a (1 - s)),  s = sigmoid(a)
+template <bool F16>
 __global__ void swiglu_bwd_kernel(const bf16* __restrict__ dh, const bf16* __restrict__ gate, const bf16* __restrict__ up,
                                   bf16* __restrict__ dgate, bf16* __restrict__ dup, long long n8) {
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n8;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     float d[8], a[8], b[8], og[8], ou[8];
-    unpack8f(reinterpret_cast<const uint4*>(dh)[i], d);
-    unpack8f(reinterpret_cast<const uint4*>(gate)[i], a);
-    unpack8f(reinterpret_cast<const uint4*>(up)[i], b);
+    unpack8t<F16>(reinterpret_cast<const uint4*>(dh)[i], d);
+    unpack8t<F16>(reinterpret_cast<const uint4*>(gate)[i], a);
+    unpack8t<F16>(reinterpret_cast<const uint4*>(up)[i], b);
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
       const float s = 1.f / (1.f + __expf(-a[k]));
       ou[k] = d[k] * a[k] * s;
       og[k] = d[k] * b[k] * s * (1.f + a[k] * (1.f - s));
     }
-    reinterpret_cast<uint4*>(dgate)[i] = pack8f(og);
-    reinterpret_cast<uint4*>(dup)[i] = pack8f(ou);
+    reinterpret_cast<uint4*>(dgate)[i] = pack8t<F16>(og);
+    reinterpret_cast<uint4*>(dup)[i] = pack8t<F16>(ou);
   }
 }
 
@@ -207,6 +202,7 @@ __global__ void swiglu_bwd_kernel(const bf16* __restrict__ dh, const bf16* __res
 // Pd and dS are written as bf16 (A operands of dV = Pd^T dO, dK = dS^T Q, dQ = dS K).  Mask semantics match the forward
 // kernel: key j visible to query i iff j <= i + (Tk - Tq) (causal) and key_mask[b][j] != 0; fully masked rows give zeros.
 // Dropout element index: (row = blockIdx.x, col = j) of stream `sid` (philox.cuh).
+template <bool F16>
 __global__ void __launch_bounds__(256) attn_softmax_bwd_kernel(const float* __restrict__ S, const float* __restrict__ dP,
                                                                bf16* __restrict__ P, bf16* __restrict__ dS, int H, int Tq,
                                                                int Tk, long long ld, float scale, int causal,
@@ -257,8 +253,8 @@ __global__ void __launch_bounds__(256) attn_softmax_bwd_kernel(const float* __re
       if (j >= Tk) break;
       const bool ok = j <= lim && (km == nullptr || km[j] != 0);
       const float pj = ok ? __expf(s[j] * scale - mx) * inv : 0.f;
-      p[j] = __float2bfloat16(pj * m[u]);
-      ds[j] = __float2bfloat16(scale * pj * (m[u] * dp[j] - D));
+      p[j] = stv<F16>(pj * m[u]);
+      ds[j] = stv<F16>(scale * pj * (m[u] * dp[j] - D));
     }
   }
 }
@@ -269,7 +265,7 @@ __global__ void __launch_bounds__(256) attn_softmax_bwd_kernel(const float* __re
 // first warp-per-row version (NV = 24, 126 registers -> 16 warps / SM) took 357 us at 14 % of the DRAM rate with
 // long-scoreboard stalls: too few loads in flight.  Hence NV is matched to Tk (17 at T = 528), the visibility mask is one
 // bit word instead of an array, and the register budget is capped so that 32 warps are resident.
-template <int NV>
+template <int NV, bool F16>
 __global__ void __launch_bounds__(256, (NV <= 20 ? 4 : 2))
 attn_softmax_bwd_warp_kernel(const float* __restrict__ S, const float* __restrict__ dP, bf16* __restrict__ P,
                              bf16* __restrict__ dS, long long rows, int H, int Tq, int Tk, long long ld, float scale,
@@ -336,14 +332,15 @@ attn_softmax_bwd_warp_kernel(const float* __restrict__ S, const float* __restric
     if (j < Tk) {
       const float pj = sv[k] * inv;
       const float mj = dc.on ? drop_mult1(dc, static_cast<uint32_t>(row), static_cast<uint32_t>(j)) : 1.0f;
-      p[j] = __float2bfloat16(pj * mj);
-      ds[j] = __float2bfloat16(scale * pj * (dv[k] - D));
+      p[j] = stv<F16>(pj * mj);
+      ds[j] = stv<F16>(scale * pj * (dv[k] - D));
     }
   }
 }
 
 // Forward half for the training step of a dropout attention (video_long_self_attention in train() mode): S fp32 ->
 // Pd = dropout(softmax(scale * S + mask)) in bf16 (the A operand of O = Pd V); same row / mask / dropout conventions.
+template <bool F16>
 __global__ void __launch_bounds__(256) attn_softmax_fwd_kernel(const float* __restrict__ S, bf16* __restrict__ P, int H, int Tq,
                                                                int Tk, long long ld, float scale, int causal,
                                                                const int* __restrict__ key_mask, float p_drop,
@@ -379,7 +376,7 @@ __global__ void __launch_bounds__(256) attn_softmax_fwd_kernel(const float* __re
       const int j = 4 * j4 + u;
       if (j >= Tk) break;
       const bool ok = j <= lim && (km == nullptr || km[j] != 0);
-      p[j] = __float2bfloat16(ok ? __expf(s[j] * scale - mx) * inv * m[u] : 0.f);
+      p[j] = stv<F16>(ok ? __expf(s[j] * scale - mx) * inv * m[u] : 0.f);
     }
     // padding columns Tk .. ld-1 are never read (the consuming GEMM's K extent is Tk)
   }
@@ -406,6 +403,7 @@ __global__ void dropout_mask_kernel(float* __restrict__ out, long long ld, int r
 // ------------------------------------------------------------------------------------------------ cross-entropy backward
 // Shifted CE of modeling.py:600-610: position t predicts labels[t+1].  dlogits[b,t,:] = (softmax(logits[b,t,:]) -
 // onehot(labels[b,t+1])) * gscale / n_valid  when t < T-1 and the label is not -100, else 0.  In place is allowed.
+template <bool F16>
 __global__ void __launch_bounds__(512) ce_bwd_kernel(const bf16* __restrict__ logits, const long long* __restrict__ labels,
                                                      bf16* __restrict__ dlogits, int T, int V,
                                                      const int* __restrict__ n_valid, float gscale,
@@ -418,27 +416,28 @@ __global__ void __launch_bounds__(512) ce_bwd_kernel(const bf16* __restrict__ lo
   long long lab = -100;
   if (t < T - 1) lab = labels[row + 1];
   if (lab < 0 || lab >= V) {
-    for (int j = threadIdx.x; j < V; j += blockDim.x) o[j] = __float2bfloat16(0.f);
+    for (int j = threadIdx.x; j < V; j += blockDim.x) o[j] = stv<F16>(0.f);
     return;
   }
   float mx = -INFINITY;
-  for (int j = threadIdx.x; j < V; j += blockDim.x) mx = fmaxf(mx, __bfloat162float(x[j]));
+  for (int j = threadIdx.x; j < V; j += blockDim.x) mx = fmaxf(mx, ldv<F16>(x[j]));
   mx = block_max(mx, sh);
   float sum = 0.f;
-  for (int j = threadIdx.x; j < V; j += blockDim.x) sum += __expf(__bfloat162float(x[j]) - mx);
+  for (int j = threadIdx.x; j < V; j += blockDim.x) sum += __expf(ldv<F16>(x[j]) - mx);
   sum = block_sum(sum, sh);
   const int nv = *n_valid;
   const float sc = gscale * (gscale_dev != nullptr ? *gscale_dev : 1.0f) / static_cast<float>(nv > 0 ? nv : 1);
   const float inv = 1.f / sum;
   for (int j = threadIdx.x; j < V; j += blockDim.x) {
-    float pj = __expf(__bfloat162float(x[j]) - mx) * inv;
+    float pj = __expf(ldv<F16>(x[j]) - mx) * inv;
     if (j == lab) pj -= 1.f;
-    o[j] = __float2bfloat16(pj * sc);
+    o[j] = stv<F16>(pj * sc);
   }
 }
 
 // ------------------------------------------------------------------------------------------------ embedding gradient
-// dtable[ids[i], :] += dx[i, :]  (bf16x2 atomics; rows with ids outside [0, vocab) are skipped)
+// dtable[ids[i], :] += dx[i, :]  (bf16x2 / half2 atomics; rows with ids outside [0, vocab) are skipped)
+template <bool F16>
 __global__ void embed_scatter_add_kernel(const bf16* __restrict__ dx, long long ldx, const long long* __restrict__ ids,
                                          long long n, int dim, int vocab, bf16* __restrict__ dtable) {
   const int half_dim = dim >> 1;
@@ -449,31 +448,44 @@ __global__ void embed_scatter_add_kernel(const bf16* __restrict__ dx, long long 
     const int c = static_cast<int>(i % half_dim);
     const long long id = ids[r];
     if (id < 0 || id >= vocab) continue;
-    const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(dx + r * ldx + 2 * c);
-    atomicAdd(reinterpret_cast<__nv_bfloat162*>(dtable + id * dim + 2 * c), v);
+    if constexpr (F16) {
+      const __half2 v = *reinterpret_cast<const __half2*>(dx + r * ldx + 2 * c);
+      atomicAdd(reinterpret_cast<__half2*>(dtable + id * dim + 2 * c), v);
+    } else {
+      const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(dx + r * ldx + 2 * c);
+      atomicAdd(reinterpret_cast<__nv_bfloat162*>(dtable + id * dim + 2 * c), v);
+    }
   }
 }
 
-// column sums of a bf16 (rows, cols) matrix into fp32 (bias gradients): out[c] += sum_r x[r, c]
+// column sums of a 16-bit (rows, cols) matrix into fp32 (bias gradients): out[c] += sum_r x[r, c]
+template <bool F16>
 __global__ void colsum_kernel(const bf16* __restrict__ x, long long ldx, int rows, int cols, float* __restrict__ out,
                               int rows_per_cta) {
   const int c = blockIdx.y * blockDim.x + threadIdx.x;
   if (c >= cols) return;
   const int r0 = blockIdx.x * rows_per_cta, r1 = min(rows, r0 + rows_per_cta);
   float acc = 0.f;
-  for (int r = r0; r < r1; ++r) acc += __bfloat162float(x[static_cast<long long>(r) * ldx + c]);
+  for (int r = r0; r < r1; ++r) acc += ldv<F16>(x[static_cast<long long>(r) * ldx + c]);
   atomicAdd(&out[c], acc);
 }
 
 // ------------------------------------------------------------------------------------------------ AdamW
-// Decoupled weight decay (Loshchilov & Hutter), fp32 master weights + moments, bf16 working copy:
-//   m = b1 m + (1-b1) g;  v = b2 v + (1-b2) g^2;  w -= lr (m/bc1 / (sqrt(v/bc2) + eps) + wd w);  p = bf16(w)
+// Decoupled weight decay (Loshchilov & Hutter), fp32 master weights + moments, 16-bit working copy and gradient in the
+// model's format:
+//   m = b1 m + (1-b1) g;  v = b2 v + (1-b2) g^2;  w -= lr (m/bc1 / (sqrt(v/bc2) + eps) + wd w);  p = 16-bit(w)
+// g is the stored gradient times gscale, or times *gmul_dev when given (the loss-scale / clipping multiplier of
+// mm_loss_scale_update).  *skip_dev != 0 (a non-finite gradient norm): the launch writes nothing.
 // 8 elements per thread and iteration: one 128-bit gradient load, two 128-bit loads / stores per fp32 state tensor, one
 // 128-bit parameter store (28 bytes of HBM traffic per parameter; the scalar kernel below reached 4.5 TB/s of it).
+template <bool F16>
 __global__ void __launch_bounds__(256) adamw_vec8_kernel(bf16* __restrict__ p, const bf16* __restrict__ g, float* __restrict__ w,
                                                          float* __restrict__ m, float* __restrict__ v, long long n8, float lr,
                                                          float b1, float b2, float eps, float wd, float inv_bc1, float inv_bc2,
-                                                         float gscale, const int* __restrict__ step_dev) {
+                                                         float gscale, const int* __restrict__ step_dev,
+                                                         const float* __restrict__ gmul_dev, const int* __restrict__ skip_dev) {
+  if (skip_dev != nullptr && *skip_dev != 0) return;
+  if (gmul_dev != nullptr) gscale = *gmul_dev;
   if (step_dev != nullptr) {
     const float t = static_cast<float>(*step_dev);
     inv_bc1 = 1.f / (1.f - powf(b1, t));
@@ -487,7 +499,7 @@ __global__ void __launch_bounds__(256) adamw_vec8_kernel(bf16* __restrict__ p, c
     float4 m0 = reinterpret_cast<const float4*>(m)[2 * i], m1 = reinterpret_cast<const float4*>(m)[2 * i + 1];
     float4 v0 = reinterpret_cast<const float4*>(v)[2 * i], v1 = reinterpret_cast<const float4*>(v)[2 * i + 1];
     float gf[8];
-    unpack8f(gu, gf);
+    unpack8t<F16>(gu, gf);
     float wf[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
     float mf[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
     float vf[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
@@ -504,13 +516,17 @@ __global__ void __launch_bounds__(256) adamw_vec8_kernel(bf16* __restrict__ p, c
     reinterpret_cast<float4*>(v)[2 * i + 1] = make_float4(vf[4], vf[5], vf[6], vf[7]);
     reinterpret_cast<float4*>(w)[2 * i] = make_float4(wf[0], wf[1], wf[2], wf[3]);
     reinterpret_cast<float4*>(w)[2 * i + 1] = make_float4(wf[4], wf[5], wf[6], wf[7]);
-    reinterpret_cast<uint4*>(p)[i] = pack8f(wf);
+    reinterpret_cast<uint4*>(p)[i] = pack8t<F16>(wf);
   }
 }
 
+template <bool F16>
 __global__ void adamw_kernel(bf16* __restrict__ p, const bf16* __restrict__ g, float* __restrict__ w, float* __restrict__ m,
                              float* __restrict__ v, long long n, float lr, float b1, float b2, float eps, float wd,
-                             float inv_bc1, float inv_bc2, float gscale, const int* __restrict__ step_dev) {
+                             float inv_bc1, float inv_bc2, float gscale, const int* __restrict__ step_dev,
+                             const float* __restrict__ gmul_dev, const int* __restrict__ skip_dev) {
+  if (skip_dev != nullptr && *skip_dev != 0) return;
+  if (gmul_dev != nullptr) gscale = *gmul_dev;
   if (step_dev != nullptr) {  // step count read on the device: the launch can be replayed from a CUDA graph
     const float t = static_cast<float>(*step_dev);
     inv_bc1 = 1.f / (1.f - powf(b1, t));
@@ -518,7 +534,7 @@ __global__ void adamw_kernel(bf16* __restrict__ p, const bf16* __restrict__ g, f
   }
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const float gi = __bfloat162float(g[i]) * gscale;
+    const float gi = ldv<F16>(g[i]) * gscale;
     const float mi = b1 * m[i] + (1.f - b1) * gi;
     const float vi = b2 * v[i] + (1.f - b2) * gi * gi;
     float wi = w[i];
@@ -526,7 +542,7 @@ __global__ void adamw_kernel(bf16* __restrict__ p, const bf16* __restrict__ g, f
     m[i] = mi;
     v[i] = vi;
     w[i] = wi;
-    p[i] = __float2bfloat16(wi);
+    p[i] = stv<F16>(wi);
   }
 }
 
@@ -539,6 +555,7 @@ __global__ void adamw_kernel(bf16* __restrict__ p, const bf16* __restrict__ g, f
 // Outputs: Pd = m . P and dS as bf16 (operands of the table-gradient GEMMs dT += Pd^T dctx~ + dS^T q~ and of dq~ = dS . table),
 // dstats[0][r] = gscale * sum_v dS_v, dstats[1][r] = gscale * p_extra * (m_V d p_extra - D) — the gradients of row_bias and
 // of the bias_k key's score (planar [2][R]).
+template <bool F16>
 __global__ void __launch_bounds__(512) align_softmax_bwd_kernel(const float* __restrict__ G, long long ldg,
                                                                 const __half* __restrict__ Pp, long long ldp,
                                                                 const float* __restrict__ inv_l,
@@ -579,8 +596,8 @@ __global__ void __launch_bounds__(512) align_softmax_bwd_kernel(const float* __r
       if (v >= V) break;
       const float pv = __half2float(pp[v]) * il;
       const float d = pv * (m[u] * (g[v] + a) - D);
-      po[v] = __float2bfloat16(pv * m[u]);
-      dso[v] = __float2bfloat16(d);
+      po[v] = stv<F16>(pv * m[u]);
+      dso[v] = stv<F16>(d);
       srow += d;
     }
   }
@@ -660,6 +677,7 @@ __global__ void cast_f16_bf16_kernel(const __half* __restrict__ x, long long ldx
 
 // Data gradient of a strided Conv1d over the token axis (col2im): dwin[(b*Lq + l), k*C + c] holds d(window l)[k, c];
 // dfeats[b, t, c] = sum over the windows l that contain token t (l*ss <= t < l*ss + kk) of dwin[b*Lq + l, (t - l*ss)*C + c].
+template <bool F16>
 __global__ void window_gather_add_kernel(const bf16* __restrict__ dwin, int B, int N, int C, int Lq, int kk, int ss,
                                          bf16* __restrict__ dfeats) {
   const long long total = static_cast<long long>(B) * N * C;
@@ -676,11 +694,109 @@ __global__ void window_gather_add_kernel(const bf16* __restrict__ dwin, int B, i
     for (int l = l_lo; l <= l_hi; ++l) {
       const int k = t - l * ss;
       if (k >= 0 && k < kk)
-        acc += __bfloat162float(dwin[(static_cast<long long>(b) * Lq + l) * (static_cast<long long>(kk) * C) +
+        acc += ldv<F16>(dwin[(static_cast<long long>(b) * Lq + l) * (static_cast<long long>(kk) * C) +
                                      static_cast<long long>(k) * C + c]);
     }
-    dfeats[i] = __float2bfloat16(acc);
+    dfeats[i] = stv<F16>(acc);
   }
+}
+
+// ------------------------------------------------------------------------------------------------ loss scaling / clipping
+// Sum of squares of a flat 16-bit gradient buffer in fp32, deterministic: a grid fixed by (n, SM count), one partial per
+// CTA (fixed-order shuffles), then one CTA sums the partials in a fixed order and adds the total into *out.  A NaN or Inf
+// element makes the total non-finite (squares are >= 0, so Inf never meets -Inf): that is the overflow test.
+constexpr int kSumsqThreads = 256, kSumsqUnroll = 4;
+
+template <bool F16>
+__global__ void __launch_bounds__(kSumsqThreads) grad_sumsq_kernel(const bf16* __restrict__ g, long long n,
+                                                                    float* __restrict__ part) {
+  __shared__ float sh[32];
+  const long long n8 = n >> 3;
+  const uint4* g8 = reinterpret_cast<const uint4*>(g);
+  const long long stride = static_cast<long long>(gridDim.x) * blockDim.x;
+  float acc = 0.f;
+  long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x;
+  // kSumsqUnroll independent 128-bit loads in flight per thread
+  for (; i + (kSumsqUnroll - 1) * stride < n8; i += kSumsqUnroll * stride) {
+    uint4 u[kSumsqUnroll];
+#pragma unroll
+    for (int k = 0; k < kSumsqUnroll; ++k) u[k] = __ldg(g8 + i + k * stride);
+#pragma unroll
+    for (int k = 0; k < kSumsqUnroll; ++k) {
+      float f[8];
+      unpack8t<F16>(u[k], f);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) acc = fmaf(f[j], f[j], acc);
+    }
+  }
+  for (; i < n8; i += stride) {
+    float f[8];
+    unpack8t<F16>(__ldg(g8 + i), f);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc = fmaf(f[j], f[j], acc);
+  }
+  if (blockIdx.x == 0 && threadIdx.x < (n & 7)) {  // the last n % 8 elements
+    const float t = ldv<F16>(g[(n8 << 3) + threadIdx.x]);
+    acc = fmaf(t, t, acc);
+  }
+  acc = block_sum(acc, sh);
+  if (threadIdx.x == 0) part[blockIdx.x] = acc;
+}
+
+__global__ void __launch_bounds__(1024) sumsq_finish_kernel(const float* __restrict__ part, int n_parts,
+                                                            float* __restrict__ out) {
+  __shared__ float sh[32];
+  float acc = 0.f;
+  for (int b = threadIdx.x; b < n_parts; b += blockDim.x) acc += part[b];
+  acc = block_sum(acc, sh);
+  if (threadIdx.x == 0) *out += acc;
+}
+
+// Dynamic loss scaling (DeepSpeed DynamicLossScaler.update_scale, consecutive_hysteresis = False) and global-norm
+// clipping (FP16_Optimizer.unscale_and_clip_grads), from the scaled gradients' sum of squares.  One thread: a few
+// dozen flops on a 48-byte state.  The arithmetic is spelled with round-to-nearest intrinsics (no FMA contraction) so
+// that a host restatement in fp32 reproduces the multiplier bit for bit.  *sumsq is consumed and reset to 0 for the
+// next step.
+__global__ void loss_scale_update_kernel(mm_loss_scale_state* __restrict__ st, float* __restrict__ sumsq, float max_norm,
+                                         int dynamic, int window, int hysteresis, float min_scale) {
+  if (threadIdx.x != 0) return;
+  const float ss = *sumsq;
+  *sumsq = 0.f;
+  const float S = st->scale;
+  const bool overflow = !isfinite(ss);
+  float mult = __frcp_rn(S);
+  if (!overflow) {
+    const float norm = __fdiv_rn(__fsqrt_rn(ss), S);
+    st->grad_norm = norm;
+    if (max_norm > 0.f) {
+      const float c = __fdiv_rn(__fadd_rn(norm, 1e-6f), max_norm);
+      mult = __frcp_rn(__fmul_rn(S, fmaxf(c, 1.f)));
+    }
+  } else {
+    st->grad_norm = ss;  // non-finite
+  }
+  st->grad_mult = mult;
+  st->skip = overflow ? 1 : 0;
+  if (overflow) {
+    st->skipped += 1;
+  } else {
+    st->step += 1;
+  }
+  if (dynamic) {
+    if (overflow) {
+      if (hysteresis == 1 || st->cur_hysteresis == 1) {
+        st->scale = fmaxf(__fmul_rn(S, 0.5f), min_scale);
+      } else {
+        st->cur_hysteresis -= 1;
+      }
+      st->last_overflow_iter = st->cur_iter;
+    } else if ((st->cur_iter - st->last_overflow_iter) % window == 0) {
+      st->cur_hysteresis = hysteresis;
+      st->scale = __fmul_rn(S, 2.f);
+    }
+    st->inv_scale = __frcp_rn(st->scale);
+  }
+  st->cur_iter += 1;
 }
 
 static inline int grid_for(long long total, int block, int cap_mult = 16) {
@@ -709,12 +825,13 @@ extern "C" int32_t mm_rmsnorm_bwd(const void* dy, const void* x, const float* rs
   if (rpc < 1) rpc = 1;
   const int grid = (rows + rpc - 1) / rpc;
   MM_REQUIRE(dg_partials == nullptr || (dg != nullptr && AL16(dg_partials)), "mm_rmsnorm_bwd: dg_partials needs dg, 16-byte aligned");
-#define MM_RB(NCH_) \
-  rmsnorm_bwd_kernel<NCH_><<<grid, 256, 0, ST(stream)>>>((const bf16*)dy, (const bf16*)x, rstd, (const bf16*)g,           \
-                                                         (const bf16*)dres, (bf16*)dx, dg, dg_partials, rows, cols, rpc)
-  if (cols <= 256 * 8) MM_RB(1);
-  else if (cols <= 256 * 8 * 2) MM_RB(2);
-  else MM_RB(4);
+#define MM_RB(NCH_, F16_) \
+  rmsnorm_bwd_kernel<NCH_, F16_><<<grid, 256, 0, ST(stream)>>>((const bf16*)dy, (const bf16*)x, rstd, (const bf16*)g,     \
+                                                               (const bf16*)dres, (bf16*)dx, dg, dg_partials, rows, cols, rpc)
+  const bool f16 = act_f16();
+  if (cols <= 256 * 8) { if (f16) MM_RB(1, true); else MM_RB(1, false); }
+  else if (cols <= 256 * 8 * 2) { if (f16) MM_RB(2, true); else MM_RB(2, false); }
+  else { if (f16) MM_RB(4, true); else MM_RB(4, false); }
 #undef MM_RB
   if (dg_partials != nullptr) dg_reduce_kernel<<<(cols + 31) / 32, 256, 0, ST(stream)>>>(dg_partials, grid, cols, dg);
   return check_launch("mm_rmsnorm_bwd");
@@ -722,7 +839,8 @@ extern "C" int32_t mm_rmsnorm_bwd(const void* dy, const void* x, const float* rs
 
 extern "C" int32_t mm_swiglu_fwd(const void* gate, const void* up, void* h, int64_t n, void* stream) {
   MM_REQUIRE(gate && up && h && n > 0 && n % 8 == 0 && AL16(gate) && AL16(up) && AL16(h), "mm_swiglu_fwd: bad arguments");
-  swiglu_fwd_kernel<<<grid_for(n / 8, 256), 256, 0, ST(stream)>>>((const bf16*)gate, (const bf16*)up, (bf16*)h, n / 8);
+  (act_f16() ? swiglu_fwd_kernel<true> : swiglu_fwd_kernel<false>)<<<grid_for(n / 8, 256), 256, 0, ST(stream)>>>(
+      (const bf16*)gate, (const bf16*)up, (bf16*)h, n / 8);
   return check_launch("mm_swiglu_fwd");
 }
 
@@ -730,8 +848,8 @@ extern "C" int32_t mm_swiglu_bwd(const void* dh, const void* gate, const void* u
                                  void* stream) {
   MM_REQUIRE(dh && gate && up && dgate && dup && n > 0 && n % 8 == 0, "mm_swiglu_bwd: bad arguments");
   MM_REQUIRE(AL16(dh) && AL16(gate) && AL16(up) && AL16(dgate) && AL16(dup), "mm_swiglu_bwd: alignment");
-  swiglu_bwd_kernel<<<grid_for(n / 8, 256), 256, 0, ST(stream)>>>((const bf16*)dh, (const bf16*)gate, (const bf16*)up,
-                                                                 (bf16*)dgate, (bf16*)dup, n / 8);
+  (act_f16() ? swiglu_bwd_kernel<true> : swiglu_bwd_kernel<false>)<<<grid_for(n / 8, 256), 256, 0, ST(stream)>>>(
+      (const bf16*)dh, (const bf16*)gate, (const bf16*)up, (bf16*)dgate, (bf16*)dup, n / 8);
   return check_launch("mm_swiglu_bwd");
 }
 
@@ -743,10 +861,12 @@ extern "C" int32_t mm_attn_softmax_bwd(const float* S, const float* dP, void* P,
   const long long rows = static_cast<long long>(B) * H * Tq;
   MM_REQUIRE(rows < (1LL << 31), "mm_attn_softmax_bwd: too many rows");
   const unsigned wgrid = static_cast<unsigned>((rows + 7) / 8);
-#define MM_SB(NV_) \
-  attn_softmax_bwd_warp_kernel<NV_><<<wgrid, 256, 0, ST(stream)>>>(S, dP, (bf16*)P, (bf16*)dS, rows, H, Tq, Tk, ld, scale, \
-                                                                   causal, key_mask, p_drop,                               \
-                                                                   (const unsigned long long*)seed_dev, sid)
+#define MM_SB(NV_)                                                                                                   \
+  (f16 ? attn_softmax_bwd_warp_kernel<NV_, true> : attn_softmax_bwd_warp_kernel<NV_, false>)<<<wgrid, 256, 0,           \
+                                                                                                ST(stream)>>>(         \
+      S, dP, (bf16*)P, (bf16*)dS, rows, H, Tq, Tk, ld, scale, causal, key_mask, p_drop,                                 \
+      (const unsigned long long*)seed_dev, sid)
+  const bool f16 = act_f16();
   const int need = (Tk + 31) / 32;  // columns per lane
   if (need <= 4) MM_SB(4);
   else if (need <= 8) MM_SB(8);
@@ -757,9 +877,9 @@ extern "C" int32_t mm_attn_softmax_bwd(const float* S, const float* dP, void* P,
   else if (need <= 24) MM_SB(24);
   else if (need <= 32) MM_SB(32);
   else
-    attn_softmax_bwd_kernel<<<static_cast<unsigned>(rows), 256, 0, ST(stream)>>>(S, dP, (bf16*)P, (bf16*)dS, H, Tq, Tk, ld,
-                                                                                 scale, causal, key_mask, p_drop,
-                                                                                 (const unsigned long long*)seed_dev, sid);
+    (f16 ? attn_softmax_bwd_kernel<true> : attn_softmax_bwd_kernel<false>)<<<static_cast<unsigned>(rows), 256, 0,
+                                                                             ST(stream)>>>(
+        S, dP, (bf16*)P, (bf16*)dS, H, Tq, Tk, ld, scale, causal, key_mask, p_drop, (const unsigned long long*)seed_dev, sid);
 #undef MM_SB
   return check_launch("mm_attn_softmax_bwd");
 }
@@ -771,9 +891,9 @@ extern "C" int32_t mm_attn_softmax_fwd(const float* S, void* P, int32_t B, int32
   MM_REQUIRE(p_drop >= 0.f && p_drop < 1.f && (p_drop == 0.f || seed_dev != nullptr), "mm_attn_softmax_fwd: dropout arguments");
   const long long rows = static_cast<long long>(B) * H * Tq;
   MM_REQUIRE(rows < (1LL << 31), "mm_attn_softmax_fwd: too many rows");
-  attn_softmax_fwd_kernel<<<static_cast<unsigned>(rows), 256, 0, ST(stream)>>>(S, (bf16*)P, H, Tq, Tk, ld, scale, causal,
-                                                                               key_mask, p_drop,
-                                                                               (const unsigned long long*)seed_dev, sid);
+  (act_f16() ? attn_softmax_fwd_kernel<true> : attn_softmax_fwd_kernel<false>)<<<static_cast<unsigned>(rows), 256, 0,
+                                                                                ST(stream)>>>(
+      S, (bf16*)P, H, Tq, Tk, ld, scale, causal, key_mask, p_drop, (const unsigned long long*)seed_dev, sid);
   return check_launch("mm_attn_softmax_fwd");
 }
 
@@ -799,8 +919,8 @@ extern "C" int32_t mm_align_dropout_fwd(const void* Pp, void* Pm, int64_t ldp, c
 extern "C" int32_t mm_ce_bwd(const void* logits, const int64_t* labels, void* dlogits, int32_t B, int32_t T, int32_t V,
                              const int32_t* n_valid, float grad_scale, const float* grad_scale_dev, void* stream) {
   MM_REQUIRE(logits && labels && dlogits && n_valid && B > 0 && T > 0 && V > 0, "mm_ce_bwd: bad arguments");
-  ce_bwd_kernel<<<B * T, 512, 0, ST(stream)>>>((const bf16*)logits, (const long long*)labels, (bf16*)dlogits, T, V, n_valid,
-                                               grad_scale, grad_scale_dev);
+  (act_f16() ? ce_bwd_kernel<true> : ce_bwd_kernel<false>)<<<B * T, 512, 0, ST(stream)>>>(
+      (const bf16*)logits, (const long long*)labels, (bf16*)dlogits, T, V, n_valid, grad_scale, grad_scale_dev);
   return check_launch("mm_ce_bwd");
 }
 
@@ -808,8 +928,9 @@ extern "C" int32_t mm_embed_scatter_add(const void* dx, int64_t ldx, const int64
                                         int32_t vocab, void* dtable, void* stream) {
   MM_REQUIRE(dx && ids && dtable && n > 0 && dim > 0 && dim % 2 == 0 && ldx % 2 == 0 && vocab > 0,
              "mm_embed_scatter_add: bad arguments");
-  embed_scatter_add_kernel<<<grid_for(n * (dim / 2), 256), 256, 0, ST(stream)>>>((const bf16*)dx, ldx, (const long long*)ids, n,
-                                                                                dim, vocab, (bf16*)dtable);
+  (act_f16() ? embed_scatter_add_kernel<true> : embed_scatter_add_kernel<false>)<<<grid_for(n * (dim / 2), 256), 256, 0,
+                                                                                  ST(stream)>>>(
+      (const bf16*)dx, ldx, (const long long*)ids, n, dim, vocab, (bf16*)dtable);
   return check_launch("mm_embed_scatter_add");
 }
 
@@ -817,27 +938,29 @@ extern "C" int32_t mm_colsum(const void* x, int64_t ldx, int32_t rows, int32_t c
   MM_REQUIRE(x && out && rows > 0 && cols > 0, "mm_colsum: bad arguments");
   int rpc = (rows + 63) / 64;
   dim3 grid((rows + rpc - 1) / rpc, (cols + 255) / 256);
-  colsum_kernel<<<grid, 256, 0, ST(stream)>>>((const bf16*)x, ldx, rows, cols, out, rpc);
+  (act_f16() ? colsum_kernel<true> : colsum_kernel<false>)<<<grid, 256, 0, ST(stream)>>>((const bf16*)x, ldx, rows, cols,
+                                                                                         out, rpc);
   return check_launch("mm_colsum");
 }
 
 extern "C" int32_t mm_adamw(void* p, const void* g, float* master, float* m, float* v, int64_t n, float lr, float beta1,
                             float beta2, float eps, float weight_decay, int32_t step, const int32_t* step_dev,
-                            float grad_scale, void* stream) {
+                            float grad_scale, const float* grad_mult_dev, const int32_t* skip_dev, void* stream) {
   MM_REQUIRE(p && g && master && m && v && n > 0 && (step > 0 || step_dev != nullptr), "mm_adamw: bad arguments");
+  const bool f16 = act_f16();
   if (step <= 0) step = 1;
   const float inv_bc1 = 1.f / (1.f - powf(beta1, static_cast<float>(step)));
   const float inv_bc2 = 1.f / (1.f - powf(beta2, static_cast<float>(step)));
   const long long n8 = (AL16(p) && AL16(g) && AL16(master) && AL16(m) && AL16(v)) ? n / 8 : 0;
   if (n8 > 0)
-    adamw_vec8_kernel<<<grid_for(n8, 256, 32), 256, 0, ST(stream)>>>((bf16*)p, (const bf16*)g, master, m, v, n8, lr, beta1,
-                                                                     beta2, eps, weight_decay, inv_bc1, inv_bc2, grad_scale,
-                                                                     step_dev);
+    (f16 ? adamw_vec8_kernel<true> : adamw_vec8_kernel<false>)<<<grid_for(n8, 256, 32), 256, 0, ST(stream)>>>(
+        (bf16*)p, (const bf16*)g, master, m, v, n8, lr, beta1, beta2, eps, weight_decay, inv_bc1, inv_bc2, grad_scale,
+        step_dev, grad_mult_dev, skip_dev);
   if (n - 8 * n8 > 0) {  // unaligned tensors / the last n % 8 elements
     const long long o = 8 * n8;
-    adamw_kernel<<<grid_for(n - o, 256), 256, 0, ST(stream)>>>((bf16*)p + o, (const bf16*)g + o, master + o, m + o, v + o, n - o,
-                                                               lr, beta1, beta2, eps, weight_decay, inv_bc1, inv_bc2, grad_scale,
-                                                               step_dev);
+    (f16 ? adamw_kernel<true> : adamw_kernel<false>)<<<grid_for(n - o, 256), 256, 0, ST(stream)>>>(
+        (bf16*)p + o, (const bf16*)g + o, master + o, m + o, v + o, n - o, lr, beta1, beta2, eps, weight_decay, inv_bc1,
+        inv_bc2, grad_scale, step_dev, grad_mult_dev, skip_dev);
   }
   return check_launch("mm_adamw");
 }
@@ -849,9 +972,9 @@ extern "C" int32_t mm_align_softmax_bwd(const float* G, int64_t ldg, const void*
   MM_REQUIRE(G && Pp && inv_l && dpsr && pe && dpe && P && dS && dstats && R > 0 && V > 0 && ldg >= V && ldp >= V && ldo >= V,
              "mm_align_softmax_bwd: bad arguments");
   MM_REQUIRE(p_drop >= 0.f && p_drop < 1.f && (p_drop == 0.f || seed_dev != nullptr), "mm_align_softmax_bwd: dropout arguments");
-  align_softmax_bwd_kernel<<<R, 512, 0, ST(stream)>>>(G, ldg, (const __half*)Pp, ldp, inv_l, dpsr, pe, dpe, gscale, (bf16*)P,
-                                                      (bf16*)dS, ldo, dstats, V, p_drop,
-                                                      (const unsigned long long*)seed_dev, sid);
+  (act_f16() ? align_softmax_bwd_kernel<true> : align_softmax_bwd_kernel<false>)<<<R, 512, 0, ST(stream)>>>(
+      G, ldg, (const __half*)Pp, ldp, inv_l, dpsr, pe, dpe, gscale, (bf16*)P, (bf16*)dS, ldo, dstats, V, p_drop,
+      (const unsigned long long*)seed_dev, sid);
   return check_launch("mm_align_softmax_bwd");
 }
 
@@ -874,7 +997,33 @@ extern "C" int32_t mm_cast_f16_bf16(const void* x, int64_t ldx, void* y, int64_t
 extern "C" int32_t mm_window_gather_add(const void* dwin, int32_t B, int32_t N, int32_t C, int32_t Lq, int32_t kk, int32_t ss,
                                         void* dfeats, void* stream) {
   MM_REQUIRE(dwin && dfeats && B > 0 && N > 0 && C > 0 && Lq > 0 && kk > 0 && ss > 0, "mm_window_gather_add: bad arguments");
-  window_gather_add_kernel<<<grid_for(static_cast<long long>(B) * N * C, 256), 256, 0, ST(stream)>>>(
-      (const bf16*)dwin, B, N, C, Lq, kk, ss, (bf16*)dfeats);
+  (act_f16() ? window_gather_add_kernel<true> : window_gather_add_kernel<false>)<<<
+      grid_for(static_cast<long long>(B) * N * C, 256), 256, 0, ST(stream)>>>((const bf16*)dwin, B, N, C, Lq, kk, ss,
+                                                                             (bf16*)dfeats);
   return check_launch("mm_window_gather_add");
+}
+
+static inline int sumsq_grid(long long n) {
+  const long long n8 = n / 8;
+  long long g = (n8 + kSumsqThreads - 1) / kSumsqThreads;
+  const long long cap = static_cast<long long>(num_sms()) * 8;
+  return static_cast<int>(g < 1 ? 1 : (g > cap ? cap : g));
+}
+
+extern "C" int32_t mm_grad_sumsq_parts(int64_t n) { return n > 0 ? sumsq_grid(n) : 0; }
+
+extern "C" int32_t mm_grad_sumsq(const void* g, int64_t n, int32_t fp16, float* out, float* partials, void* stream) {
+  MM_REQUIRE(g && out && partials && n > 0 && AL16(g), "mm_grad_sumsq: bad arguments (g 16-byte aligned, n > 0)");
+  const int grid = sumsq_grid(n);
+  (fp16 ? grad_sumsq_kernel<true> : grad_sumsq_kernel<false>)<<<grid, kSumsqThreads, 0, ST(stream)>>>((const bf16*)g, n,
+                                                                                                      partials);
+  sumsq_finish_kernel<<<1, 1024, 0, ST(stream)>>>(partials, grid, out);
+  return check_launch("mm_grad_sumsq");
+}
+
+extern "C" int32_t mm_loss_scale_update(mm_loss_scale_state* state, float* sumsq, float max_norm, int32_t dynamic,
+                                        int32_t window, int32_t hysteresis, float min_scale, void* stream) {
+  MM_REQUIRE(state && sumsq && window > 0 && hysteresis > 0 && min_scale > 0.f, "mm_loss_scale_update: bad arguments");
+  loss_scale_update_kernel<<<1, 32, 0, ST(stream)>>>(state, sumsq, max_norm, dynamic, window, hysteresis, min_scale);
+  return check_launch("mm_loss_scale_update");
 }

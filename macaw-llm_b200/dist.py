@@ -87,11 +87,13 @@ def init_nccl(device=None) -> bool:
 
 
 def nccl_allreduce_(t: torch.Tensor, average: bool = True) -> None:
-    """In-place all-reduce of a contiguous bf16 / fp32 CUDA tensor on torch's CURRENT stream through mm_nccl_allreduce."""
+    """In-place all-reduce of a contiguous bf16 / fp16 / fp32 CUDA tensor on torch's CURRENT stream through
+    mm_nccl_allreduce."""
     from . import _lib
 
-    assert _NCCL_READY and t.is_cuda and t.is_contiguous() and t.dtype in (torch.bfloat16, torch.float32)
-    rc = _lib.load().mm_nccl_allreduce(t.data_ptr(), t.numel(), int(t.dtype == torch.float32), int(average),
+    codes = {torch.bfloat16: 0, torch.float32: 1, torch.float16: 2}
+    assert _NCCL_READY and t.is_cuda and t.is_contiguous() and t.dtype in codes
+    rc = _lib.load().mm_nccl_allreduce(t.data_ptr(), t.numel(), codes[t.dtype], int(average),
                                        torch.cuda.current_stream().cuda_stream)
     if rc != 0:
         raise RuntimeError(f"mm_nccl_allreduce failed: {_lib.last_error()}")

@@ -659,7 +659,6 @@ def attention_train_fwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, *, sc
     for n, t in (("q", q), ("k", k), ("v", v)):
         _cuda(t, ACT(), n)
         assert t.dim() == 4 and t.stride(3) == 1
-    assert ACT() == torch.bfloat16, "the training step computes in bf16"
     B, Tq, H, hd = q.shape
     Tk = k.shape[1]
     dev = q.device
@@ -780,16 +779,53 @@ def colsum(x: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
 
 def adamw(p: torch.Tensor, g: torch.Tensor, master: torch.Tensor, m: torch.Tensor, v: torch.Tensor, *, lr: float,
           beta1: float, beta2: float, eps: float, weight_decay: float, step: int, grad_scale: float = 1.0,
-          step_dev: Optional[torch.Tensor] = None) -> None:
+          step_dev: Optional[torch.Tensor] = None, grad_mult_dev: Optional[torch.Tensor] = None,
+          skip_dev: Optional[torch.Tensor] = None) -> None:
+    """Fused AdamW on one tensor (p, g in the activation format).  grad_mult_dev: device fp32 scalar replacing grad_scale;
+    skip_dev: device int32 scalar, non-zero = write nothing (see mm_adamw)."""
     _cuda(p, ACT(), "p"); _cuda(g, ACT(), "g")
     assert p.is_contiguous() and g.is_contiguous() and master.numel() == p.numel()
     _check(_lib.load().mm_adamw(p.data_ptr(), g.data_ptr(), master.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(),
                                 float(lr), float(beta1), float(beta2), float(eps), float(weight_decay), int(step),
-                                _ptr(step_dev), float(grad_scale), _stream()), "mm_adamw")
+                                _ptr(step_dev), float(grad_scale), _ptr(grad_mult_dev), _ptr(skip_dev), _stream()),
+           "mm_adamw")
+
+
+def grad_sumsq_parts(n: int) -> int:
+    """Size of the fp32 partials workspace mm_grad_sumsq uses for n elements (on the current device)."""
+    return int(_lib.load().mm_grad_sumsq_parts(int(n)))
+
+
+def grad_sumsq(g: torch.Tensor, out: torch.Tensor, partials: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out (device fp32 scalar) += sum(g.float() ** 2) over a contiguous bf16 / fp16 tensor, deterministically; a NaN / Inf
+    element makes the result non-finite (mm_grad_sumsq)."""
+    _cuda(g, None, "g"); _cuda(out, torch.float32, "out")
+    assert g.dtype in _16BIT and g.is_contiguous() and out.numel() == 1
+    n = g.numel()
+    if partials is None:
+        partials = torch.empty((grad_sumsq_parts(n),), device=g.device, dtype=torch.float32)
+    assert partials.dtype == torch.float32 and partials.numel() >= grad_sumsq_parts(n)
+    _check(_lib.load().mm_grad_sumsq(g.data_ptr(), n, int(g.dtype == _F16), out.data_ptr(), partials.data_ptr(), _stream()),
+           "mm_grad_sumsq")
+    return out
+
+
+LOSS_SCALE_STATE_WORDS = 12  # sizeof(mm_loss_scale_state) / 4
+
+
+def loss_scale_update(state: torch.Tensor, sumsq: torch.Tensor, *, max_norm: Optional[float], dynamic: bool,
+                      window: int, hysteresis: int, min_scale: float) -> None:
+    """One step of the device loss scaler / clipper over `state` (int32 (12,) tensor laid out as mm_loss_scale_state);
+    consumes and zeroes `sumsq` (mm_loss_scale_update)."""
+    _cuda(state, torch.int32, "state"); _cuda(sumsq, torch.float32, "sumsq")
+    assert state.numel() == LOSS_SCALE_STATE_WORDS and state.is_contiguous() and sumsq.numel() == 1
+    _check(_lib.load().mm_loss_scale_update(state.data_ptr(), sumsq.data_ptr(), float(max_norm or 0.0), int(dynamic),
+                                            int(window), int(hysteresis), float(min_scale), _stream()),
+           "mm_loss_scale_update")
 
 
 def cast_bf16(x: torch.Tensor) -> torch.Tensor:
-    """fp16 contiguous tensor -> bf16 copy (mm_cast_f16_bf16): the alignment backward runs in bf16 (gradient range)."""
+    """fp16 contiguous tensor -> bf16 copy (mm_cast_f16_bf16): the alignment backward of a bf16 model runs in bf16."""
     _cuda(x, _F16, "x")
     assert x.is_contiguous()
     cols = x.shape[-1]
@@ -816,7 +852,7 @@ def align_dropout_fwd(P_unnorm: torch.Tensor, inv_l: torch.Tensor, pe: torch.Ten
 
 def align_softmax_bwd(G: torch.Tensor, P_unnorm: torch.Tensor, inv_l: torch.Tensor, dpsr: torch.Tensor, pe: torch.Tensor,
                       dpe: torch.Tensor, gscale: float, V: int, dropout=None):
-    """-> (Pd bf16 (R, ldp), dS bf16 (R, ldp), dstats fp32 (2, R)); see mm_align_softmax_bwd."""
+    """-> (Pd (R, ldp), dS (R, ldp) in the activation format, dstats fp32 (2, R)); see mm_align_softmax_bwd."""
     _cuda(G, torch.float32, "G"); _cuda(P_unnorm, _F16, "P")
     R, ldp = P_unnorm.shape
     assert G.shape[0] == R and G.stride(1) == 1 and P_unnorm.stride(1) == 1
@@ -844,10 +880,10 @@ def head_weighted_colsum(x: torch.Tensor, w: torch.Tensor, head_dim: int, out: t
 
 
 def window_gather_add(dwin: torch.Tensor, B: int, N: int, C: int, Lq: int, kk: int, ss: int) -> torch.Tensor:
-    """Conv1d data gradient: dwin (B*Lq, kk*C) bf16 -> dfeats (B, N, C) bf16 (mm_window_gather_add)."""
-    _cuda(dwin, torch.bfloat16, "dwin")
+    """Conv1d data gradient: dwin (B*Lq, kk*C) -> dfeats (B, N, C), both in the activation format (mm_window_gather_add)."""
+    _cuda(dwin, ACT(), "dwin")
     assert dwin.is_contiguous() and dwin.shape == (B * Lq, kk * C)
-    out = torch.empty((B, N, C), device=dwin.device, dtype=torch.bfloat16)
+    out = torch.empty((B, N, C), device=dwin.device, dtype=ACT())
     _check(_lib.load().mm_window_gather_add(dwin.data_ptr(), B, N, C, Lq, kk, ss, out.data_ptr(), _stream()),
            "mm_window_gather_add")
     return out
