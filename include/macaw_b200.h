@@ -8,8 +8,11 @@
  *
  * Conventions
  *   - every function returns 0 on success, non-zero on error; mm_last_error() returns a message for the
- *     calling thread.  No exceptions cross this boundary and nothing here calls cudaMalloc.
- *   - all pointers are DEVICE pointers owned by the caller (torch's caching allocator in practice).
+ *     calling thread.  No exceptions cross this boundary and nothing here calls cudaMalloc.  mm_host_alloc /
+ *     mm_host_free (page-locked host memory for optimizer state) are the library's ONLY allocating entries; they are
+ *     called when an optimizer is set up and torn down, never inside a training step.
+ *   - all pointers are DEVICE pointers owned by the caller (torch's caching allocator in practice), or device aliases of
+ *     mm_host_alloc memory where a function says so.
  *   - `stream` is a cudaStream_t passed as void*; all calls are asynchronous and never synchronise.
  *   - "bf16" means 16-bit bfloat16 storage, row-major unless a leading dimension says otherwise; all
  *     accumulation is fp32.
@@ -385,6 +388,18 @@ int32_t mm_colsum(const void* x, int64_t ldx, int32_t rows, int32_t cols, float*
 int32_t mm_adamw(void* p, const void* g, float* master, float* m, float* v, int64_t n, float lr, float beta1, float beta2,
                  float eps, float weight_decay, int32_t step, const int32_t* step_dev, float grad_scale,
                  const float* grad_mult_dev, const int32_t* skip_dev, void* stream);
+/* AdamW state in page-locked host memory (DeepSpeed's offload_optimizer {device: cpu, pin_memory: true}, but updated by
+ * the GPU: no CPU execution path).  mm_host_alloc allocates exactly `bytes` with cudaHostAllocMapped |
+ * cudaHostAllocPortable and returns the host pointer and its device alias (cudaHostGetDevicePointer); it fails when the
+ * current device cannot map host memory.  mm_host_free releases a block by its host pointer.
+ * mm_adamw_host: mm_adamw's arguments and arithmetic (bit-identical results: one shared per-element update), with
+ * master / m / v device aliases of mm_host_alloc memory (16-byte aligned) and p / g in device memory (8-byte aligned).
+ * The launch is bound by the PCIe link: lane-contiguous 16-byte accesses, 24 B of host traffic per element. */
+int32_t mm_adamw_host(void* p, const void* g, float* master, float* m, float* v, int64_t n, float lr, float beta1,
+                      float beta2, float eps, float weight_decay, int32_t step, const int32_t* step_dev, float grad_scale,
+                      const float* grad_mult_dev, const int32_t* skip_dev, void* stream);
+int32_t mm_host_alloc(int64_t bytes, void** host_ptr, void** dev_ptr);
+int32_t mm_host_free(void* host_ptr);
 
 /* ------------------------------------------------------------------------------------------------ loss scaling / clipping
  * fp16 training with dynamic loss scaling and global gradient-norm clipping, on the device and free of host syncs (the

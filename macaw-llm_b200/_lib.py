@@ -145,6 +145,10 @@ SIGNATURES = {
     "mm_colsum": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_vp]),
     "mm_adamw": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_i32, c_vp, c_f32, c_vp,
                          c_vp, c_vp]),
+    "mm_adamw_host": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_i32, c_vp, c_f32,
+                              c_vp, c_vp, c_vp]),
+    "mm_host_alloc": (c_i32, [c_i64, C.POINTER(c_vp), C.POINTER(c_vp)]),
+    "mm_host_free": (c_i32, [c_vp]),
     "mm_grad_sumsq_parts": (c_i32, [c_i64]),
     "mm_grad_sumsq": (c_i32, [c_vp, c_i64, c_i32, c_vp, c_vp, c_vp]),
     "mm_loss_scale_update": (c_i32, [c_vp, c_vp, c_f32, c_i32, c_i32, c_i32, c_f32, c_vp]),
@@ -163,7 +167,7 @@ SIGNATURES = {
 }
 
 _lib = None
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 
 def load(build_if_missing: bool = True) -> C.CDLL:

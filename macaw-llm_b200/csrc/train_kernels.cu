@@ -476,6 +476,41 @@ __global__ void colsum_kernel(const bf16* __restrict__ x, long long ldx, int row
 //   m = b1 m + (1-b1) g;  v = b2 v + (1-b2) g^2;  w -= lr (m/bc1 / (sqrt(v/bc2) + eps) + wd w);  p = 16-bit(w)
 // g is the stored gradient times gscale, or times *gmul_dev when given (the loss-scale / clipping multiplier of
 // mm_loss_scale_update).  *skip_dev != 0 (a non-finite gradient norm): the launch writes nothing.
+// The three AdamW kernels below share the device-side scalars and the per-element update through these two functions, so
+// that a tensor gives bit-identical results whichever kernel (and wherever its state) it is updated with.
+//
+// Device scalars of one launch: the gradient multiplier (*gmul_dev when given) and the bias corrections (from *step_dev
+// when given: graph-replayed steps).  Returns false when *skip_dev says the step is skipped.
+__device__ __forceinline__ bool adamw_scalars(float b1, float b2, float& inv_bc1, float& inv_bc2, float& gscale,
+                                              const int* __restrict__ step_dev, const float* __restrict__ gmul_dev,
+                                              const int* __restrict__ skip_dev) {
+  if (skip_dev != nullptr && *skip_dev != 0) return false;
+  if (gmul_dev != nullptr) gscale = *gmul_dev;
+  if (step_dev != nullptr) {
+    const float t = static_cast<float>(*step_dev);
+    inv_bc1 = 1.f / (1.f - powf(b1, t));
+    inv_bc2 = 1.f / (1.f - powf(b2, t));
+  }
+  return true;
+}
+// One element: g the stored gradient, c1 = 1 - b1, c2 = 1 - b2.
+//   m = b1 m + c1 gi;  v = b2 v + c2 gi^2;  w -= lr (m/bc1 / (sqrt(v/bc2) + eps) + wd w)
+// Spelled with round-to-nearest intrinsics, so that the rounding does not depend on how the compiler contracts the
+// expression in each loop.  Left to it, the 8-wide kernel fused the second moment as fma(gi, c2 gi, b2 v) and the scalar
+// kernel as fma(v, b2, (c2 gi) gi): mm_adamw updates the elements below 8 * (n / 8) of an aligned tensor one way and the
+// rest the other.  V8 selects between those two forms, exactly as the compiler had chosen them (the two kernels' machine
+// code is unchanged), and the host-state kernel uses each on the elements mm_adamw would, so that its results are
+// bit-identical.
+template <bool V8>
+__device__ __forceinline__ void adamw_elem(float g, float& w, float& m, float& v, float lr, float b1, float b2, float c1,
+                                           float c2, float eps, float wd, float inv_bc1, float inv_bc2, float gscale) {
+  const float gi = __fmul_rn(g, gscale);
+  m = __fmaf_rn(m, b1, __fmul_rn(c1, gi));
+  v = V8 ? __fmaf_rn(gi, __fmul_rn(c2, gi), __fmul_rn(b2, v)) : __fmaf_rn(v, b2, __fmul_rn(__fmul_rn(c2, gi), gi));
+  const float r = __fmaf_rn(w, wd, __fdiv_rn(__fmul_rn(m, inv_bc1), __fadd_rn(__fsqrt_rn(__fmul_rn(v, inv_bc2)), eps)));
+  w = __fmaf_rn(-r, lr, w);
+}
+
 // 8 elements per thread and iteration: one 128-bit gradient load, two 128-bit loads / stores per fp32 state tensor, one
 // 128-bit parameter store (28 bytes of HBM traffic per parameter; the scalar kernel below reached 4.5 TB/s of it).
 template <bool F16>
@@ -484,13 +519,7 @@ __global__ void __launch_bounds__(256) adamw_vec8_kernel(bf16* __restrict__ p, c
                                                          float b1, float b2, float eps, float wd, float inv_bc1, float inv_bc2,
                                                          float gscale, const int* __restrict__ step_dev,
                                                          const float* __restrict__ gmul_dev, const int* __restrict__ skip_dev) {
-  if (skip_dev != nullptr && *skip_dev != 0) return;
-  if (gmul_dev != nullptr) gscale = *gmul_dev;
-  if (step_dev != nullptr) {
-    const float t = static_cast<float>(*step_dev);
-    inv_bc1 = 1.f / (1.f - powf(b1, t));
-    inv_bc2 = 1.f / (1.f - powf(b2, t));
-  }
+  if (!adamw_scalars(b1, b2, inv_bc1, inv_bc2, gscale, step_dev, gmul_dev, skip_dev)) return;
   const float c1 = 1.f - b1, c2 = 1.f - b2;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n8;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -504,12 +533,7 @@ __global__ void __launch_bounds__(256) adamw_vec8_kernel(bf16* __restrict__ p, c
     float mf[8] = {m0.x, m0.y, m0.z, m0.w, m1.x, m1.y, m1.z, m1.w};
     float vf[8] = {v0.x, v0.y, v0.z, v0.w, v1.x, v1.y, v1.z, v1.w};
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float gi = gf[j] * gscale;
-      mf[j] = b1 * mf[j] + c1 * gi;
-      vf[j] = b2 * vf[j] + c2 * gi * gi;
-      wf[j] -= lr * (mf[j] * inv_bc1 / (sqrtf(vf[j] * inv_bc2) + eps) + wd * wf[j]);
-    }
+    for (int j = 0; j < 8; ++j) adamw_elem<true>(gf[j], wf[j], mf[j], vf[j], lr, b1, b2, c1, c2, eps, wd, inv_bc1, inv_bc2, gscale);
     reinterpret_cast<float4*>(m)[2 * i] = make_float4(mf[0], mf[1], mf[2], mf[3]);
     reinterpret_cast<float4*>(m)[2 * i + 1] = make_float4(mf[4], mf[5], mf[6], mf[7]);
     reinterpret_cast<float4*>(v)[2 * i] = make_float4(vf[0], vf[1], vf[2], vf[3]);
@@ -525,20 +549,63 @@ __global__ void adamw_kernel(bf16* __restrict__ p, const bf16* __restrict__ g, f
                              float* __restrict__ v, long long n, float lr, float b1, float b2, float eps, float wd,
                              float inv_bc1, float inv_bc2, float gscale, const int* __restrict__ step_dev,
                              const float* __restrict__ gmul_dev, const int* __restrict__ skip_dev) {
-  if (skip_dev != nullptr && *skip_dev != 0) return;
-  if (gmul_dev != nullptr) gscale = *gmul_dev;
-  if (step_dev != nullptr) {  // step count read on the device: the launch can be replayed from a CUDA graph
-    const float t = static_cast<float>(*step_dev);
-    inv_bc1 = 1.f / (1.f - powf(b1, t));
-    inv_bc2 = 1.f / (1.f - powf(b2, t));
-  }
+  if (!adamw_scalars(b1, b2, inv_bc1, inv_bc2, gscale, step_dev, gmul_dev, skip_dev)) return;
+  const float c1 = 1.f - b1, c2 = 1.f - b2;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const float gi = ldv<F16>(g[i]) * gscale;
-    const float mi = b1 * m[i] + (1.f - b1) * gi;
-    const float vi = b2 * v[i] + (1.f - b2) * gi * gi;
-    float wi = w[i];
-    wi -= lr * (mi * inv_bc1 / (sqrtf(vi * inv_bc2) + eps) + wd * wi);
+    float wi = w[i], mi = m[i], vi = v[i];
+    adamw_elem<false>(ldv<F16>(g[i]), wi, mi, vi, lr, b1, b2, c1, c2, eps, wd, inv_bc1, inv_bc2, gscale);
+    m[i] = mi;
+    v[i] = vi;
+    w[i] = wi;
+    p[i] = stv<F16>(wi);
+  }
+}
+
+// The same update with master / m / v in page-locked host memory (device aliases of mm_host_alloc blocks, reached over
+// PCIe) and p / g in HBM.  The link is the bottleneck, so the access pattern is laid out for it: lane l owns the 4
+// consecutive elements 4 (i0 + l) .. +3, so every warp instruction on w, m or v moves 512 contiguous bytes and each byte of
+// host state is read once and written once (24 B of host traffic per element); the gradient is loaded as 4 x 16 bit
+// (8 B) and the parameter stored as 8 B.  All loads of an iteration are issued before the arithmetic; the last n % 4
+// elements are a scalar loop of the first CTA.  Elements below n_v8 take the 8-wide kernel's form of the update, the others
+// the scalar kernel's (adamw_elem): n_v8 = 8 * (n / 8) when mm_adamw would run the 8-wide kernel on these tensors, else 0.
+template <bool F16>
+__global__ void __launch_bounds__(256) adamw_host_kernel(bf16* __restrict__ p, const bf16* __restrict__ g, float* __restrict__ w,
+                                                         float* __restrict__ m, float* __restrict__ v, long long n,
+                                                         long long n_v8, float lr,
+                                                         float b1, float b2, float eps, float wd, float inv_bc1, float inv_bc2,
+                                                         float gscale, const int* __restrict__ step_dev,
+                                                         const float* __restrict__ gmul_dev, const int* __restrict__ skip_dev) {
+  if (!adamw_scalars(b1, b2, inv_bc1, inv_bc2, gscale, step_dev, gmul_dev, skip_dev)) return;
+  const float c1 = 1.f - b1, c2 = 1.f - b2;
+  const long long n4 = n >> 2;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const uint2 gu = __ldg(reinterpret_cast<const uint2*>(g) + i);
+    const float4 w4 = reinterpret_cast<const float4*>(w)[i];
+    const float4 m4 = reinterpret_cast<const float4*>(m)[i];
+    const float4 v4 = reinterpret_cast<const float4*>(v)[i];
+    float gf[4], wf[4] = {w4.x, w4.y, w4.z, w4.w}, mf[4] = {m4.x, m4.y, m4.z, m4.w}, vf[4] = {v4.x, v4.y, v4.z, v4.w};
+    unpack2<F16>(gu.x, gf[0], gf[1]);
+    unpack2<F16>(gu.y, gf[2], gf[3]);
+    if (4 * i < n_v8) {  // (n_v8 is a multiple of 8: a group of 4 lies entirely on one side)
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        adamw_elem<true>(gf[j], wf[j], mf[j], vf[j], lr, b1, b2, c1, c2, eps, wd, inv_bc1, inv_bc2, gscale);
+    } else {
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        adamw_elem<false>(gf[j], wf[j], mf[j], vf[j], lr, b1, b2, c1, c2, eps, wd, inv_bc1, inv_bc2, gscale);
+    }
+    reinterpret_cast<float4*>(m)[i] = make_float4(mf[0], mf[1], mf[2], mf[3]);
+    reinterpret_cast<float4*>(v)[i] = make_float4(vf[0], vf[1], vf[2], vf[3]);
+    reinterpret_cast<float4*>(w)[i] = make_float4(wf[0], wf[1], wf[2], wf[3]);
+    reinterpret_cast<uint2*>(p)[i] = make_uint2(pack2<F16>(wf[0], wf[1]), pack2<F16>(wf[2], wf[3]));
+  }
+  if (blockIdx.x == 0 && threadIdx.x < (n & 3)) {
+    const long long i = (n4 << 2) + threadIdx.x;
+    float wi = w[i], mi = m[i], vi = v[i];
+    adamw_elem<false>(ldv<F16>(g[i]), wi, mi, vi, lr, b1, b2, c1, c2, eps, wd, inv_bc1, inv_bc2, gscale);
     m[i] = mi;
     v[i] = vi;
     w[i] = wi;
@@ -963,6 +1030,65 @@ extern "C" int32_t mm_adamw(void* p, const void* g, float* master, float* m, flo
         inv_bc2, grad_scale, step_dev, grad_mult_dev, skip_dev);
   }
   return check_launch("mm_adamw");
+}
+
+#define AL8(p) ((reinterpret_cast<uintptr_t>(p) & 7) == 0)
+
+extern "C" int32_t mm_adamw_host(void* p, const void* g, float* master, float* m, float* v, int64_t n, float lr, float beta1,
+                                 float beta2, float eps, float weight_decay, int32_t step, const int32_t* step_dev,
+                                 float grad_scale, const float* grad_mult_dev, const int32_t* skip_dev, void* stream) {
+  MM_REQUIRE(p && g && master && m && v && n > 0 && (step > 0 || step_dev != nullptr), "mm_adamw_host: bad arguments");
+  MM_REQUIRE(AL16(master) && AL16(m) && AL16(v) && AL8(p) && AL8(g),
+             "mm_adamw_host: alignment (master / m / v 16-byte, p / g 8-byte aligned)");
+  const bool f16 = act_f16();
+  if (step <= 0) step = 1;
+  const float inv_bc1 = 1.f / (1.f - powf(beta1, static_cast<float>(step)));
+  const float inv_bc2 = 1.f / (1.f - powf(beta2, static_cast<float>(step)));
+  const long long n_v8 = (AL16(p) && AL16(g)) ? n / 8 * 8 : 0;  // the elements mm_adamw gives to adamw_vec8_kernel
+  (f16 ? adamw_host_kernel<true> : adamw_host_kernel<false>)<<<grid_for(n / 4 > 0 ? n / 4 : 1, 256), 256, 0, ST(stream)>>>(
+      (bf16*)p, (const bf16*)g, master, m, v, n, n_v8, lr, beta1, beta2, eps, weight_decay, inv_bc1, inv_bc2, grad_scale,
+      step_dev, grad_mult_dev, skip_dev);
+  return check_launch("mm_adamw_host");
+}
+
+extern "C" int32_t mm_host_alloc(int64_t bytes, void** host_ptr, void** dev_ptr) {
+  MM_REQUIRE(bytes > 0 && host_ptr && dev_ptr, "mm_host_alloc: bad arguments (bytes > 0, non-null outputs)");
+  *host_ptr = nullptr;
+  *dev_ptr = nullptr;
+  int dev = 0, can_map = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&can_map, cudaDevAttrCanMapHostMemory, dev);
+  if (e != cudaSuccess) {
+    set_error("mm_host_alloc: no usable CUDA device: %s", cudaGetErrorString(e));
+    return 2;
+  }
+  MM_REQUIRE(can_map, "mm_host_alloc: device %d cannot map page-locked host memory", dev);
+  void* h = nullptr;
+  e = cudaHostAlloc(&h, static_cast<size_t>(bytes), cudaHostAllocMapped | cudaHostAllocPortable);
+  if (e != cudaSuccess) {
+    set_error("mm_host_alloc: cudaHostAlloc(%lld bytes) failed: %s", static_cast<long long>(bytes), cudaGetErrorString(e));
+    return 2;
+  }
+  void* d = nullptr;
+  e = cudaHostGetDevicePointer(&d, h, 0);
+  if (e != cudaSuccess) {
+    cudaFreeHost(h);
+    set_error("mm_host_alloc: cudaHostGetDevicePointer failed: %s", cudaGetErrorString(e));
+    return 2;
+  }
+  *host_ptr = h;
+  *dev_ptr = d;
+  return 0;
+}
+
+extern "C" int32_t mm_host_free(void* host_ptr) {
+  MM_REQUIRE(host_ptr, "mm_host_free: null pointer");
+  const cudaError_t e = cudaFreeHost(host_ptr);
+  if (e != cudaSuccess) {
+    set_error("mm_host_free: cudaFreeHost failed: %s", cudaGetErrorString(e));
+    return 2;
+  }
+  return 0;
 }
 
 extern "C" int32_t mm_align_softmax_bwd(const float* G, int64_t ldg, const void* Pp, int64_t ldp, const float* inv_l,

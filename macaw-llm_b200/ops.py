@@ -791,6 +791,61 @@ def adamw(p: torch.Tensor, g: torch.Tensor, master: torch.Tensor, m: torch.Tenso
            "mm_adamw")
 
 
+class HostBlock:
+    """`nbytes` of page-locked host memory mapped into the device's address space (mm_host_alloc): AdamW state that does not
+    fit in HBM, updated in place by `adamw_host` over PCIe.  `view(offset, numel)` is a CPU float32 tensor over part of the
+    block.  The block lives until `free()` (idempotent); views must not be used after it."""
+
+    def __init__(self, nbytes: int):
+        if nbytes <= 0:
+            raise ValueError("HostBlock: nbytes must be > 0")
+        h, d = C.c_void_p(), C.c_void_p()
+        _check(_lib.load().mm_host_alloc(int(nbytes), C.byref(h), C.byref(d)), "mm_host_alloc")
+        self.nbytes, self.host, self.dev = int(nbytes), int(h.value), int(d.value)
+        self._flat = torch.frombuffer((C.c_char * self.nbytes).from_address(self.host), dtype=torch.uint8)
+
+    def view(self, offset: int, numel: int) -> torch.Tensor:
+        """float32 CPU tensor of `numel` elements at byte `offset` (16-byte aligned)."""
+        if offset % 16 or offset < 0 or offset + 4 * numel > self.nbytes:
+            raise ValueError(f"HostBlock.view: [{offset}, {offset + 4 * numel}) is not a 16-byte aligned range of the block")
+        return self._flat[offset:offset + 4 * numel].view(torch.float32)
+
+    def dev_ptr(self, t: torch.Tensor) -> int:
+        """Device alias of the data of `t`, a contiguous float32 view of this block."""
+        off = t.data_ptr() - self.host
+        if t.device.type != "cpu" or t.dtype != torch.float32 or not t.is_contiguous() or off < 0 or \
+                off + 4 * t.numel() > self.nbytes:
+            raise ValueError("HostBlock.dev_ptr: not a contiguous float32 view of this block")
+        return self.dev + off
+
+    def free(self) -> None:
+        if self.host:
+            self._flat = None
+            _check(_lib.load().mm_host_free(self.host), "mm_host_free")
+            self.host = self.dev = 0
+
+
+def host_alloc(nbytes: int) -> HostBlock:
+    """Exactly `nbytes` of mapped, page-locked host memory (mm_host_alloc; not torch's pinned allocator, which rounds every
+    block up to a power of two)."""
+    return HostBlock(nbytes)
+
+
+def adamw_host(p: torch.Tensor, g: torch.Tensor, master: torch.Tensor, m: torch.Tensor, v: torch.Tensor, *,
+               block: HostBlock, lr: float, beta1: float, beta2: float, eps: float, weight_decay: float, step: int,
+               grad_scale: float = 1.0, step_dev: Optional[torch.Tensor] = None,
+               grad_mult_dev: Optional[torch.Tensor] = None, skip_dev: Optional[torch.Tensor] = None) -> None:
+    """`adamw` with master / m / v CPU float32 views of `block` (host memory, reached by the kernel over PCIe); p, g on the
+    device.  Bit-identical to `adamw` on device copies of the same state (mm_adamw_host)."""
+    _cuda(p, ACT(), "p"); _cuda(g, ACT(), "g")
+    assert p.is_contiguous() and g.is_contiguous() and master.numel() == m.numel() == v.numel() == p.numel()
+    _check(_lib.load().mm_adamw_host(p.data_ptr(), g.data_ptr(), block.dev_ptr(master), block.dev_ptr(m), block.dev_ptr(v),
+                                     p.numel(), float(lr), float(beta1), float(beta2), float(eps), float(weight_decay),
+                                     int(step), _ptr(step_dev), float(grad_scale), _ptr(grad_mult_dev), _ptr(skip_dev),
+                                     _stream()),
+           "mm_adamw_host")
+
+
 def grad_sumsq_parts(n: int) -> int:
     """Size of the fp32 partials workspace mm_grad_sumsq uses for n elements (on the current device)."""
     return int(_lib.load().mm_grad_sumsq_parts(int(n)))

@@ -8,3 +8,6 @@ timeout 500 compute-sanitizer --tool racecheck --error-exitcode 9 --print-limit 
 timeout 900 compute-sanitizer --tool memcheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_train_fp16_gpu.py -q -x -m gpu -k "not gradients_vs_oracle and not cuda_graph and not skipped and not beyond" --timeout 850 --timeout-method=thread 2>&1 | tail -12
 echo "memcheck (fp16 training) rc=$?"
 timeout 600 compute-sanitizer --tool racecheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_train_fp16_gpu.py -q -x -m gpu -k "rmsnorm_swiglu or ce_backward or grad_sumsq_vs or loss_scale_update" --timeout 550 --timeout-method=thread 2>&1 | tail -8
+# AdamW with host-resident state (mm_host_alloc + mm_adamw_host; the 32000 x 4096 kernel case is left out: 1.6 GB of host state)
+timeout 600 compute-sanitizer --tool memcheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_optimizer_offload_gpu.py -q -x -m gpu -k "not 131072000" --timeout 550 --timeout-method=thread 2>&1 | tail -8
+echo "memcheck (host-state AdamW) rc=$?"
