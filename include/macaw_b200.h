@@ -384,10 +384,12 @@ int32_t mm_colsum(const void* x, int64_t ldx, int32_t rows, int32_t cols, float*
  * (graph-replayed training steps).  grad_mult_dev (nullable): a device fp32 multiplier that replaces grad_scale — the
  * unscale-and-clip factor of mm_loss_scale_update (DeepSpeed FP16_Optimizer.unscale_and_clip_grads).  skip_dev
  * (nullable): a device int; when non-zero the launch writes nothing (p, master, m, v unchanged: the overflow-skipped
- * step of DeepSpeed's fp16 optimizer).  With both null the behaviour is that of ABI 3. */
+ * step of DeepSpeed's fp16 optimizer).  With both null the behaviour is that of ABI 3.  lr_dev (nullable, ABI 6): a device
+ * fp32 lr that replaces `lr` — the output of mm_lr_schedule; every AdamW kernel (8-wide, scalar, host-state) reads it
+ * alike.  With lr_dev null the results are those of ABI 5, bit for bit. */
 int32_t mm_adamw(void* p, const void* g, float* master, float* m, float* v, int64_t n, float lr, float beta1, float beta2,
                  float eps, float weight_decay, int32_t step, const int32_t* step_dev, float grad_scale,
-                 const float* grad_mult_dev, const int32_t* skip_dev, void* stream);
+                 const float* grad_mult_dev, const int32_t* skip_dev, const float* lr_dev, void* stream);
 /* AdamW state in page-locked host memory (DeepSpeed's offload_optimizer {device: cpu, pin_memory: true}, but updated by
  * the GPU: no CPU execution path).  mm_host_alloc allocates exactly `bytes` with cudaHostAllocMapped |
  * cudaHostAllocPortable and returns the host pointer and its device alias (cudaHostGetDevicePointer); it fails when the
@@ -397,7 +399,7 @@ int32_t mm_adamw(void* p, const void* g, float* master, float* m, float* v, int6
  * The launch is bound by the PCIe link: lane-contiguous 16-byte accesses, 24 B of host traffic per element. */
 int32_t mm_adamw_host(void* p, const void* g, float* master, float* m, float* v, int64_t n, float lr, float beta1,
                       float beta2, float eps, float weight_decay, int32_t step, const int32_t* step_dev, float grad_scale,
-                      const float* grad_mult_dev, const int32_t* skip_dev, void* stream);
+                      const float* grad_mult_dev, const int32_t* skip_dev, const float* lr_dev, void* stream);
 int32_t mm_host_alloc(int64_t bytes, void** host_ptr, void** dev_ptr);
 int32_t mm_host_free(void* host_ptr);
 
@@ -437,6 +439,29 @@ typedef struct mm_loss_scale_state {
  *   keeps S (a kernel cannot raise) and the step is skipped.  Then cur_iter += 1.  *sumsq is reset to 0. */
 int32_t mm_loss_scale_update(mm_loss_scale_state* state, float* sumsq, float max_norm, int32_t dynamic, int32_t window,
                              int32_t hysteresis, float min_scale, void* stream);
+
+/* ------------------------------------------------------------------------------------------------ learning-rate schedule
+ * The lr of every AdamW step computed on the device from the AdamW step counter, so the whole step stays one CUDA graph
+ * with no host sync.  Reference: train.sh `--learning_rate 3e-5 --warmup_ratio 0.03 --lr_scheduler_type cosine`; HF
+ * Trainer builds the schedule (transformers.optimization get_*_schedule_with_warmup, a LambdaLR) and DeepSpeed steps it
+ * only on steps it does not skip for overflow.
+ *
+ * mm_lr_schedule: one single-thread launch per optimizer step, AFTER mm_loss_scale_update (or the increment of the
+ * caller's step counter when there is neither scaler nor clipping) and BEFORE the AdamW launches, which get lr_out as
+ * their lr_dev.  With t = *step_dev (mm_loss_scale_state.step, the counter the bias corrections use: t-th applied update)
+ * and n = max(t - 1, 0), in double:
+ *   *lr_out = fp32(base_lr * lambda(n)),  W = warmup_steps, N = training_steps,
+ *   kind 0 linear:                lambda = n / max(1, W) for n < W, else max(0, (N - n) / max(1, N - W))
+ *   kind 1 cosine:                lambda = n / max(1, W) for n < W, else max(0, 0.5 (1 + cos(pi (n - W) / max(1, N - W))))
+ *                                 (not clamped past N: it rises again, as HF's)
+ *   kind 2 constant_with_warmup:  lambda = n / max(1, W) for n < W, else 1
+ * The first applied update therefore runs at lr 0 when W > 0 (HF's LambdaLR): m and v move, master and p do not.  Skip
+ * rule: an overflow-skipped step does not advance t, so it does not advance the schedule (the launch rewrites the lr of the
+ * latest applied update, which the skipped AdamW launches do not use); after k skips the schedule runs k steps behind the
+ * iteration count.  Gradient-accumulation micro-batches do not advance it either.  Arguments are checked before any CUDA
+ * call: non-null pointers, kind in 0..2, 0 <= W <= N, N >= 1. */
+int32_t mm_lr_schedule(const int32_t* step_dev, double base_lr, int32_t kind, int32_t warmup_steps, int32_t training_steps,
+                       float* lr_out, void* stream);
 
 /* Backward of the absorbed alignment attention through its (V + 2)-key softmax (reference: autograd of
  * nn.MultiheadAttention, modeling.py:986-987 / 1007-1008 / 1025-1026).  See train_kernels.cu for the formulas. */

@@ -144,9 +144,10 @@ SIGNATURES = {
     "mm_embed_scatter_add": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_vp, c_vp]),
     "mm_colsum": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_vp]),
     "mm_adamw": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_i32, c_vp, c_f32, c_vp,
-                         c_vp, c_vp]),
+                         c_vp, c_vp, c_vp]),
     "mm_adamw_host": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_i64, c_f32, c_f32, c_f32, c_f32, c_f32, c_i32, c_vp, c_f32,
-                              c_vp, c_vp, c_vp]),
+                              c_vp, c_vp, c_vp, c_vp]),
+    "mm_lr_schedule": (c_i32, [c_vp, C.c_double, c_i32, c_i32, c_i32, c_vp, c_vp]),
     "mm_host_alloc": (c_i32, [c_i64, C.POINTER(c_vp), C.POINTER(c_vp)]),
     "mm_host_free": (c_i32, [c_vp]),
     "mm_grad_sumsq_parts": (c_i32, [c_i64]),
@@ -166,8 +167,31 @@ SIGNATURES = {
     "mm_ce_loss": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp]),
 }
 
+# Nullable pointers added to an entry after it first shipped, just before its final `stream` argument: a Python call may
+# leave them out and they are passed as NULL, with the caller's last argument still going to `stream`, so code written
+# against the shorter argument list keeps its meaning.
+#   mm_adamw / mm_adamw_host: lr_dev (ABI 6, between skip_dev and stream), NULL = the `lr` argument
+NULLABLE_BEFORE_STREAM = {"mm_adamw": 1, "mm_adamw_host": 1}
+
 _lib = None
-ABI_VERSION = 5
+ABI_VERSION = 6
+
+
+class _NullableBeforeStream:
+    """A bound entry whose `n_opt` pointer arguments before the final `stream` default to NULL: a call that is k <= n_opt
+    arguments short gets k NULLs inserted before its last argument, which stays the stream."""
+
+    def __init__(self, fn, n_opt: int):
+        self._fn, self._n_opt = fn, n_opt
+
+    def __call__(self, *args):
+        n = len(self._fn.argtypes)
+        if n - self._n_opt <= len(args) < n:
+            args = args[:-1] + (None,) * (n - len(args)) + args[-1:]
+        return self._fn(*args)
+
+    def __getattr__(self, name):
+        return getattr(self._fn, name)
 
 
 def load(build_if_missing: bool = True) -> C.CDLL:
@@ -191,6 +215,8 @@ def load(build_if_missing: bool = True) -> C.CDLL:
         fn = getattr(lib, name)  # AttributeError here == ABI drift; fail loudly
         fn.restype = res
         fn.argtypes = args
+        if name in NULLABLE_BEFORE_STREAM:
+            setattr(lib, name, _NullableBeforeStream(fn, NULLABLE_BEFORE_STREAM[name]))
     got = lib.mm_build_hash().decode()
     if got != want or lib.mm_abi_version() != ABI_VERSION:
         raise RuntimeError(f"libmacaw_b200.so was built from other sources (library {got}, csrc {want}; ABI "

@@ -479,13 +479,15 @@ __global__ void colsum_kernel(const bf16* __restrict__ x, long long ldx, int row
 // The three AdamW kernels below share the device-side scalars and the per-element update through these two functions, so
 // that a tensor gives bit-identical results whichever kernel (and wherever its state) it is updated with.
 //
-// Device scalars of one launch: the gradient multiplier (*gmul_dev when given) and the bias corrections (from *step_dev
-// when given: graph-replayed steps).  Returns false when *skip_dev says the step is skipped.
-__device__ __forceinline__ bool adamw_scalars(float b1, float b2, float& inv_bc1, float& inv_bc2, float& gscale,
+// Device scalars of one launch: the gradient multiplier (*gmul_dev when given), the lr (*lr_dev when given: the output of
+// mm_lr_schedule) and the bias corrections (from *step_dev when given: graph-replayed steps).  Returns false when
+// *skip_dev says the step is skipped.
+__device__ __forceinline__ bool adamw_scalars(float b1, float b2, float& inv_bc1, float& inv_bc2, float& gscale, float& lr,
                                               const int* __restrict__ step_dev, const float* __restrict__ gmul_dev,
-                                              const int* __restrict__ skip_dev) {
+                                              const int* __restrict__ skip_dev, const float* __restrict__ lr_dev) {
   if (skip_dev != nullptr && *skip_dev != 0) return false;
   if (gmul_dev != nullptr) gscale = *gmul_dev;
+  if (lr_dev != nullptr) lr = *lr_dev;
   if (step_dev != nullptr) {
     const float t = static_cast<float>(*step_dev);
     inv_bc1 = 1.f / (1.f - powf(b1, t));
@@ -518,8 +520,9 @@ __global__ void __launch_bounds__(256) adamw_vec8_kernel(bf16* __restrict__ p, c
                                                          float* __restrict__ m, float* __restrict__ v, long long n8, float lr,
                                                          float b1, float b2, float eps, float wd, float inv_bc1, float inv_bc2,
                                                          float gscale, const int* __restrict__ step_dev,
-                                                         const float* __restrict__ gmul_dev, const int* __restrict__ skip_dev) {
-  if (!adamw_scalars(b1, b2, inv_bc1, inv_bc2, gscale, step_dev, gmul_dev, skip_dev)) return;
+                                                         const float* __restrict__ gmul_dev, const int* __restrict__ skip_dev,
+                                                         const float* __restrict__ lr_dev) {
+  if (!adamw_scalars(b1, b2, inv_bc1, inv_bc2, gscale, lr, step_dev, gmul_dev, skip_dev, lr_dev)) return;
   const float c1 = 1.f - b1, c2 = 1.f - b2;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n8;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -548,8 +551,9 @@ template <bool F16>
 __global__ void adamw_kernel(bf16* __restrict__ p, const bf16* __restrict__ g, float* __restrict__ w, float* __restrict__ m,
                              float* __restrict__ v, long long n, float lr, float b1, float b2, float eps, float wd,
                              float inv_bc1, float inv_bc2, float gscale, const int* __restrict__ step_dev,
-                             const float* __restrict__ gmul_dev, const int* __restrict__ skip_dev) {
-  if (!adamw_scalars(b1, b2, inv_bc1, inv_bc2, gscale, step_dev, gmul_dev, skip_dev)) return;
+                             const float* __restrict__ gmul_dev, const int* __restrict__ skip_dev,
+                             const float* __restrict__ lr_dev) {
+  if (!adamw_scalars(b1, b2, inv_bc1, inv_bc2, gscale, lr, step_dev, gmul_dev, skip_dev, lr_dev)) return;
   const float c1 = 1.f - b1, c2 = 1.f - b2;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -575,8 +579,9 @@ __global__ void __launch_bounds__(256) adamw_host_kernel(bf16* __restrict__ p, c
                                                          long long n_v8, float lr,
                                                          float b1, float b2, float eps, float wd, float inv_bc1, float inv_bc2,
                                                          float gscale, const int* __restrict__ step_dev,
-                                                         const float* __restrict__ gmul_dev, const int* __restrict__ skip_dev) {
-  if (!adamw_scalars(b1, b2, inv_bc1, inv_bc2, gscale, step_dev, gmul_dev, skip_dev)) return;
+                                                         const float* __restrict__ gmul_dev, const int* __restrict__ skip_dev,
+                                                         const float* __restrict__ lr_dev) {
+  if (!adamw_scalars(b1, b2, inv_bc1, inv_bc2, gscale, lr, step_dev, gmul_dev, skip_dev, lr_dev)) return;
   const float c1 = 1.f - b1, c2 = 1.f - b2;
   const long long n4 = n >> 2;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n4;
@@ -866,6 +871,30 @@ __global__ void loss_scale_update_kernel(mm_loss_scale_state* __restrict__ st, f
   st->cur_iter += 1;
 }
 
+// Learning-rate schedule of HF Trainer (transformers/optimization.py: linear, cosine with num_cycles 0.5 and
+// min_lr_rate 0, constant_with_warmup), evaluated in double as HF does in Python: *lr_out = fp32(base_lr * lambda(n)),
+// n = max(*step_dev - 1, 0) the scheduler steps taken before the AdamW update that reads it.  One thread.
+__global__ void lr_schedule_kernel(const int* __restrict__ step_dev, double base_lr, int kind, int warmup, int total,
+                                   float* __restrict__ lr_out) {
+  const long long t = *step_dev;
+  const long long n = t > 1 ? t - 1 : 0;
+  double lam;
+  if (n < warmup) {
+    lam = static_cast<double>(n) / static_cast<double>(warmup > 1 ? warmup : 1);
+  } else if (kind == 2) {  // constant_with_warmup
+    lam = 1.0;
+  } else {
+    const double span = static_cast<double>(total - warmup > 1 ? total - warmup : 1);
+    if (kind == 0) {  // linear
+      lam = fmax(0.0, static_cast<double>(total - n) / span);
+    } else {  // cosine: past `total` it rises again, as HF's does
+      const double progress = static_cast<double>(n - warmup) / span;
+      lam = fmax(0.0, 0.5 * (1.0 + cos(3.141592653589793 * progress)));
+    }
+  }
+  *lr_out = __double2float_rn(__dmul_rn(base_lr, lam));
+}
+
 static inline int grid_for(long long total, int block, int cap_mult = 16) {
   long long g = (total + block - 1) / block;
   const long long cap = static_cast<long long>(num_sms()) * cap_mult;
@@ -1012,7 +1041,8 @@ extern "C" int32_t mm_colsum(const void* x, int64_t ldx, int32_t rows, int32_t c
 
 extern "C" int32_t mm_adamw(void* p, const void* g, float* master, float* m, float* v, int64_t n, float lr, float beta1,
                             float beta2, float eps, float weight_decay, int32_t step, const int32_t* step_dev,
-                            float grad_scale, const float* grad_mult_dev, const int32_t* skip_dev, void* stream) {
+                            float grad_scale, const float* grad_mult_dev, const int32_t* skip_dev, const float* lr_dev,
+                            void* stream) {
   MM_REQUIRE(p && g && master && m && v && n > 0 && (step > 0 || step_dev != nullptr), "mm_adamw: bad arguments");
   const bool f16 = act_f16();
   if (step <= 0) step = 1;
@@ -1022,12 +1052,12 @@ extern "C" int32_t mm_adamw(void* p, const void* g, float* master, float* m, flo
   if (n8 > 0)
     (f16 ? adamw_vec8_kernel<true> : adamw_vec8_kernel<false>)<<<grid_for(n8, 256, 32), 256, 0, ST(stream)>>>(
         (bf16*)p, (const bf16*)g, master, m, v, n8, lr, beta1, beta2, eps, weight_decay, inv_bc1, inv_bc2, grad_scale,
-        step_dev, grad_mult_dev, skip_dev);
+        step_dev, grad_mult_dev, skip_dev, lr_dev);
   if (n - 8 * n8 > 0) {  // unaligned tensors / the last n % 8 elements
     const long long o = 8 * n8;
     (f16 ? adamw_kernel<true> : adamw_kernel<false>)<<<grid_for(n - o, 256), 256, 0, ST(stream)>>>(
         (bf16*)p + o, (const bf16*)g + o, master + o, m + o, v + o, n - o, lr, beta1, beta2, eps, weight_decay, inv_bc1,
-        inv_bc2, grad_scale, step_dev, grad_mult_dev, skip_dev);
+        inv_bc2, grad_scale, step_dev, grad_mult_dev, skip_dev, lr_dev);
   }
   return check_launch("mm_adamw");
 }
@@ -1036,7 +1066,8 @@ extern "C" int32_t mm_adamw(void* p, const void* g, float* master, float* m, flo
 
 extern "C" int32_t mm_adamw_host(void* p, const void* g, float* master, float* m, float* v, int64_t n, float lr, float beta1,
                                  float beta2, float eps, float weight_decay, int32_t step, const int32_t* step_dev,
-                                 float grad_scale, const float* grad_mult_dev, const int32_t* skip_dev, void* stream) {
+                                 float grad_scale, const float* grad_mult_dev, const int32_t* skip_dev, const float* lr_dev,
+                                 void* stream) {
   MM_REQUIRE(p && g && master && m && v && n > 0 && (step > 0 || step_dev != nullptr), "mm_adamw_host: bad arguments");
   MM_REQUIRE(AL16(master) && AL16(m) && AL16(v) && AL8(p) && AL8(g),
              "mm_adamw_host: alignment (master / m / v 16-byte, p / g 8-byte aligned)");
@@ -1047,7 +1078,7 @@ extern "C" int32_t mm_adamw_host(void* p, const void* g, float* master, float* m
   const long long n_v8 = (AL16(p) && AL16(g)) ? n / 8 * 8 : 0;  // the elements mm_adamw gives to adamw_vec8_kernel
   (f16 ? adamw_host_kernel<true> : adamw_host_kernel<false>)<<<grid_for(n / 4 > 0 ? n / 4 : 1, 256), 256, 0, ST(stream)>>>(
       (bf16*)p, (const bf16*)g, master, m, v, n, n_v8, lr, beta1, beta2, eps, weight_decay, inv_bc1, inv_bc2, grad_scale,
-      step_dev, grad_mult_dev, skip_dev);
+      step_dev, grad_mult_dev, skip_dev, lr_dev);
   return check_launch("mm_adamw_host");
 }
 
@@ -1152,4 +1183,15 @@ extern "C" int32_t mm_loss_scale_update(mm_loss_scale_state* state, float* sumsq
   MM_REQUIRE(state && sumsq && window > 0 && hysteresis > 0 && min_scale > 0.f, "mm_loss_scale_update: bad arguments");
   loss_scale_update_kernel<<<1, 32, 0, ST(stream)>>>(state, sumsq, max_norm, dynamic, window, hysteresis, min_scale);
   return check_launch("mm_loss_scale_update");
+}
+
+extern "C" int32_t mm_lr_schedule(const int32_t* step_dev, double base_lr, int32_t kind, int32_t warmup_steps,
+                                  int32_t training_steps, float* lr_out, void* stream) {
+  MM_REQUIRE(step_dev && lr_out, "mm_lr_schedule: bad arguments (null pointer)");
+  MM_REQUIRE(kind >= 0 && kind <= 2, "mm_lr_schedule: unknown kind %d (0 linear, 1 cosine, 2 constant_with_warmup)", kind);
+  MM_REQUIRE(warmup_steps >= 0 && training_steps >= 1 && warmup_steps <= training_steps,
+             "mm_lr_schedule: bad step counts (0 <= warmup_steps <= training_steps, training_steps >= 1; got %d, %d)",
+             warmup_steps, training_steps);
+  lr_schedule_kernel<<<1, 1, 0, ST(stream)>>>(step_dev, base_lr, kind, warmup_steps, training_steps, lr_out);
+  return check_launch("mm_lr_schedule");
 }

@@ -780,15 +780,32 @@ def colsum(x: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
 def adamw(p: torch.Tensor, g: torch.Tensor, master: torch.Tensor, m: torch.Tensor, v: torch.Tensor, *, lr: float,
           beta1: float, beta2: float, eps: float, weight_decay: float, step: int, grad_scale: float = 1.0,
           step_dev: Optional[torch.Tensor] = None, grad_mult_dev: Optional[torch.Tensor] = None,
-          skip_dev: Optional[torch.Tensor] = None) -> None:
+          skip_dev: Optional[torch.Tensor] = None, lr_dev: Optional[torch.Tensor] = None) -> None:
     """Fused AdamW on one tensor (p, g in the activation format).  grad_mult_dev: device fp32 scalar replacing grad_scale;
-    skip_dev: device int32 scalar, non-zero = write nothing (see mm_adamw)."""
+    skip_dev: device int32 scalar, non-zero = write nothing; lr_dev: device fp32 scalar replacing lr (the output of
+    `lr_schedule`) (see mm_adamw)."""
     _cuda(p, ACT(), "p"); _cuda(g, ACT(), "g")
     assert p.is_contiguous() and g.is_contiguous() and master.numel() == p.numel()
     _check(_lib.load().mm_adamw(p.data_ptr(), g.data_ptr(), master.data_ptr(), m.data_ptr(), v.data_ptr(), p.numel(),
                                 float(lr), float(beta1), float(beta2), float(eps), float(weight_decay), int(step),
-                                _ptr(step_dev), float(grad_scale), _ptr(grad_mult_dev), _ptr(skip_dev), _stream()),
+                                _ptr(step_dev), float(grad_scale), _ptr(grad_mult_dev), _ptr(skip_dev), _ptr(lr_dev),
+                                _stream()),
            "mm_adamw")
+
+
+LR_SCHEDULE_KINDS = {"linear": 0, "cosine": 1, "constant_with_warmup": 2}  # mm_lr_schedule's `kind`
+
+
+def lr_schedule(step_dev: torch.Tensor, lr_out: torch.Tensor, *, base_lr: float, kind: str, warmup_steps: int,
+                training_steps: int) -> None:
+    """lr_out (device fp32 scalar) = fp32(base_lr * lambda(t - 1)), t = *step_dev the AdamW step counter after it has
+    advanced, lambda HF's multiplier of schedule `kind` (LR_SCHEDULE_KINDS); one single-thread launch (mm_lr_schedule)."""
+    _cuda(step_dev, torch.int32, "step_dev"); _cuda(lr_out, torch.float32, "lr_out")
+    assert step_dev.numel() == 1 and lr_out.numel() == 1
+    if kind not in LR_SCHEDULE_KINDS:
+        raise ValueError(f"lr_schedule: unknown kind {kind!r}; supported: {', '.join(LR_SCHEDULE_KINDS)}")
+    _check(_lib.load().mm_lr_schedule(step_dev.data_ptr(), float(base_lr), LR_SCHEDULE_KINDS[kind], int(warmup_steps),
+                                      int(training_steps), lr_out.data_ptr(), _stream()), "mm_lr_schedule")
 
 
 class HostBlock:
@@ -834,7 +851,8 @@ def host_alloc(nbytes: int) -> HostBlock:
 def adamw_host(p: torch.Tensor, g: torch.Tensor, master: torch.Tensor, m: torch.Tensor, v: torch.Tensor, *,
                block: HostBlock, lr: float, beta1: float, beta2: float, eps: float, weight_decay: float, step: int,
                grad_scale: float = 1.0, step_dev: Optional[torch.Tensor] = None,
-               grad_mult_dev: Optional[torch.Tensor] = None, skip_dev: Optional[torch.Tensor] = None) -> None:
+               grad_mult_dev: Optional[torch.Tensor] = None, skip_dev: Optional[torch.Tensor] = None,
+               lr_dev: Optional[torch.Tensor] = None) -> None:
     """`adamw` with master / m / v CPU float32 views of `block` (host memory, reached by the kernel over PCIe); p, g on the
     device.  Bit-identical to `adamw` on device copies of the same state (mm_adamw_host)."""
     _cuda(p, ACT(), "p"); _cuda(g, ACT(), "g")
@@ -842,7 +860,7 @@ def adamw_host(p: torch.Tensor, g: torch.Tensor, master: torch.Tensor, m: torch.
     _check(_lib.load().mm_adamw_host(p.data_ptr(), g.data_ptr(), block.dev_ptr(master), block.dev_ptr(m), block.dev_ptr(v),
                                      p.numel(), float(lr), float(beta1), float(beta2), float(eps), float(weight_decay),
                                      int(step), _ptr(step_dev), float(grad_scale), _ptr(grad_mult_dev), _ptr(skip_dev),
-                                     _stream()),
+                                     _ptr(lr_dev), _stream()),
            "mm_adamw_host")
 
 

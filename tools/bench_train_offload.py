@@ -93,7 +93,7 @@ def kernels(n: int, reps: int) -> dict:
         v.zero_()
         lib = _lib.load()
         args = lambda: (p.data_ptr(), g.data_ptr(), blk.dev_ptr(w), blk.dev_ptr(m), blk.dev_ptr(v), n, 1e-5, 0.9,  # noqa: E731
-                        0.999, 1e-8, 0.0, 1, None, 1.0, None, None, ops._stream())
+                        0.999, 1e-8, 0.0, 1, None, 1.0, None, None, None, ops._stream())
         old = lambda: ops._check(lib.mm_adamw(*args()), "mm_adamw")  # noqa: E731
         new = lambda: ops._check(lib.mm_adamw_host(*args()), "mm_adamw_host")  # noqa: E731
         t = {"mm_adamw_on_alias": [], "mm_adamw_host": []}

@@ -11,3 +11,6 @@ timeout 600 compute-sanitizer --tool racecheck --error-exitcode 9 --print-limit 
 # AdamW with host-resident state (mm_host_alloc + mm_adamw_host; the 32000 x 4096 kernel case is left out: 1.6 GB of host state)
 timeout 600 compute-sanitizer --tool memcheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_optimizer_offload_gpu.py -q -x -m gpu -k "not 131072000" --timeout 550 --timeout-method=thread 2>&1 | tail -8
 echo "memcheck (host-state AdamW) rc=$?"
+# learning-rate schedule (mm_lr_schedule, lr_dev of the AdamW kernels; the tiny-model graph test is left out)
+timeout 600 compute-sanitizer --tool memcheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_lr_schedule_gpu.py -q -x -m gpu -k "not cuda_graph" --timeout 550 --timeout-method=thread 2>&1 | tail -8
+echo "memcheck (lr schedule) rc=$?"
