@@ -686,7 +686,12 @@ def attention_bwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, do: torch.T
     """Backward of mm_attn_fwd composed from wgmma GEMMs: S = q k^T and dP = dO v^T (fp32, batched over (b, h)), one
     row-wise softmax-backward kernel (P, dS in bf16), then dV = P^T dO, dK = dS^T q (MN-major A), dQ = dS k.
     q / do (B, Tq, H, hd), k / v (B, Tk, H, hd): bf16 views with unit head-dim stride.  Returns contiguous dq, dk, dv.
-    dropout = (p, seed_dev, sid): backward of attention_train_fwd with the same mask (regenerated, not stored)."""
+    dropout = (p, seed_dev, sid): backward of attention_train_fwd with the same mask (regenerated, not stored).
+
+    fp16: dS is stored UNSCALED, as torch's autograd keeps it (the scale goes into the fp32 score GEMM's alpha and into the
+    dK / dQ GEMMs' alpha).  With the scale folded in, scale * P (dP - D) of a flat softmax row (P ~ 1 / Tk) under a small
+    upstream gradient lands in fp16's subnormal range: a 1 / sqrt(96) scale there cost video_long_self_attention's key-side
+    gradients 5-7x the error of torch's fp16 autograd.  bf16 keeps the folded scale (no subnormals at these magnitudes)."""
     for n, t in (("q", q), ("k", k), ("v", v), ("do", do)):
         _cuda(t, ACT(), n)
         assert t.dim() == 4 and t.stride(3) == 1
@@ -700,13 +705,16 @@ def attention_bwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, do: torch.T
     def bat(t):  # (lda, head stride, sample stride) of a (B, T, H, hd) view
         return dict(ld=t.stride(1), bs=t.stride(2), bs2=t.stride(0))
 
-    def scores(a, b, out):
+    # (alpha of the score GEMM, scale passed to the softmax kernel, alpha of the dK / dQ GEMMs)
+    s_alpha, k_scale, g_alpha = (float(scale), 1.0, float(scale)) if ACT() == _F16 else (1.0, float(scale), 1.0)
+
+    def scores(a, b, out, alpha=1.0):
         sa, sb = bat(a), bat(b)
         gemm_raw(M=Tq, N=Tk, K=hd, batch=H, batch2=B, A=a.data_ptr(), lda=sa["ld"], a_bs=sa["bs"], a_bs2=sa["bs2"],
                  B=b.data_ptr(), ldb=sb["ld"], b_bs=sb["bs"], b_bs2=sb["bs2"], Cout=out.data_ptr(), ldc=Tp, c_bs=Tq * Tp,
-                 c_bs2=H * Tq * Tp, c_fp32=True)
+                 c_bs2=H * Tq * Tp, c_fp32=True, alpha=alpha)
 
-    scores(q, k, S)
+    scores(q, k, S, s_alpha)
     scores(do, v, dP)
     P = torch.empty((B, H, Tq, Tp), device=dev, dtype=ACT())
     dS = torch.empty((B, H, Tq, Tp), device=dev, dtype=ACT())
@@ -714,25 +722,25 @@ def attention_bwd(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, do: torch.T
         _cuda(key_mask, torch.int32, "key_mask")
     pd, seed, sid = _drop_args(dropout)
     _check(_lib.load().mm_attn_softmax_bwd(S.data_ptr(), dP.data_ptr(), P.data_ptr(), dS.data_ptr(), B, H, Tq, Tk, Tp,
-                                           float(scale), int(causal), _ptr(key_mask), pd, seed, sid, _stream()),
+                                           k_scale, int(causal), _ptr(key_mask), pd, seed, sid, _stream()),
            "mm_attn_softmax_bwd")
     del S, dP
     dq = torch.empty((B, Tq, H, hd), device=dev, dtype=ACT())
     dk = torch.empty((B, Tk, H, hd), device=dev, dtype=ACT())
     dv = torch.empty((B, Tk, H, hd), device=dev, dtype=ACT())
 
-    def pt_x(p_, x_, out):  # out_bh (Tk, hd) = p_bh^T (Tk x Tq) @ x_bh (Tq, hd)
+    def pt_x(p_, x_, out, alpha=1.0):  # out_bh (Tk, hd) = alpha * p_bh^T (Tk x Tq) @ x_bh (Tq, hd)
         sx, so = bat(x_), bat(out)
         gemm_raw(M=Tk, N=hd, K=Tq, batch=H, batch2=B, A=p_.data_ptr(), lda=Tp, a_bs=Tq * Tp, a_bs2=H * Tq * Tp,
                  a_mn_major=True, B=x_.data_ptr(), ldb=sx["ld"], b_bs=sx["bs"], b_bs2=sx["bs2"], b_mn_major=True,
-                 Cout=out.data_ptr(), ldc=so["ld"], c_bs=so["bs"], c_bs2=so["bs2"])
+                 Cout=out.data_ptr(), ldc=so["ld"], c_bs=so["bs"], c_bs2=so["bs2"], alpha=alpha)
 
     pt_x(P, do, dv)
-    pt_x(dS, q, dk)
+    pt_x(dS, q, dk, g_alpha)
     sk, so = bat(k), bat(dq)
     gemm_raw(M=Tq, N=hd, K=Tk, batch=H, batch2=B, A=dS.data_ptr(), lda=Tp, a_bs=Tq * Tp, a_bs2=H * Tq * Tp,
              B=k.data_ptr(), ldb=sk["ld"], b_bs=sk["bs"], b_bs2=sk["bs2"], b_mn_major=True, Cout=dq.data_ptr(),
-             ldc=so["ld"], c_bs=so["bs"], c_bs2=so["bs2"])
+             ldc=so["ld"], c_bs=so["bs"], c_bs2=so["bs2"], alpha=g_alpha)
     return dq, dk, dv
 
 

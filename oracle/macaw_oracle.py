@@ -105,7 +105,7 @@ def mha_forward(query: Tensor, key: Tensor, value: Tensor, w: _SD, num_heads: in
     q = q.reshape(Lq, B * num_heads, hd).transpose(0, 1)
     k = k.reshape(S + 1, B * num_heads, hd).transpose(0, 1)
     v = v.reshape(S + 1, B * num_heads, hd).transpose(0, 1)
-    zeros = torch.zeros(B * num_heads, 1, hd, dtype=k.dtype)
+    zeros = torch.zeros(B * num_heads, 1, hd, dtype=k.dtype, device=k.device)
     k = torch.cat([k, zeros], dim=1)
     v = torch.cat([v, zeros], dim=1)
     q = q * (1.0 / math.sqrt(hd))

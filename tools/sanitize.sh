@@ -14,3 +14,9 @@ echo "memcheck (host-state AdamW) rc=$?"
 # learning-rate schedule (mm_lr_schedule, lr_dev of the AdamW kernels; the tiny-model graph test is left out)
 timeout 600 compute-sanitizer --tool memcheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_lr_schedule_gpu.py -q -x -m gpu -k "not cuda_graph" --timeout 550 --timeout-method=thread 2>&1 | tail -8
 echo "memcheck (lr schedule) rc=$?"
+# alignment-backward kernels (softmax backward, dropout forward, head-weighted column sums, col2im, f16 -> bf16 cast; the
+# real-width model test is left out); both row kernels reduce through shared memory
+timeout 900 compute-sanitizer --tool memcheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_align_backward_gpu.py -q -x -m gpu -k "not real_width" --timeout 850 --timeout-method=thread 2>&1 | tail -8
+echo "memcheck (alignment backward kernels) rc=$?"
+timeout 600 compute-sanitizer --tool racecheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_align_backward_gpu.py -q -x -m gpu -k "(align_softmax_bwd and (V32000-R97-drop-extra or V519 or V4097)) or (align_dropout_fwd and (V32000-R97-0.1 or V519))" --timeout 550 --timeout-method=thread 2>&1 | tail -8
+echo "racecheck (alignment backward kernels) rc=$?"
