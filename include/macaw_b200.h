@@ -154,6 +154,10 @@ int32_t mm_gemm_plan(const mm_gemm_args* args, mm_gemm_schedule* plan);
 /* Stream-K policy of the process: 0 never, 1 when the saved MMA time exceeds the hand-over cost (default; environment
  * MACAW_B200_GEMM_STREAMK), 2 whenever the schedule allows (tests).  mode < 0 only queries.  Returns the previous mode. */
 int32_t mm_gemm_streamk_mode(int32_t mode);
+/* Epilogue-overlap policy of the process: 0 the consumer warpgroups run each tile's epilogue themselves, 1 a dedicated
+ * epilogue warpgroup runs it while they start the next tile (default; environment MACAW_B200_GEMM_OVERLAP).  Outputs are
+ * bit-identical in both modes.  mode < 0 only queries.  Returns the previous mode. */
+int32_t mm_gemm_overlap_mode(int32_t mode);
 /* bytes of mm_gemm_args.sk_workspace on the current device */
 int64_t mm_gemm_streamk_workspace_bytes(void);
 

@@ -126,6 +126,7 @@ SIGNATURES = {
     "mm_kv_append": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp]),
     "mm_gemm_streamk_workspace_bytes": (c_i64, []),
     "mm_gemm_streamk_mode": (c_i32, [c_i32]),
+    "mm_gemm_overlap_mode": (c_i32, [c_i32]),
     "mm_thin_fused": (c_i32, [C.POINTER(ThinArgs), c_vp]),
     "mm_thin_reduce": (c_i32, [c_vp, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp]),
     "mm_argmax_rows": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_vp]),

@@ -4,6 +4,13 @@
 //   warps 0..7  : two consumer warpgroups; warpgroup g issues wgmma for rows 64 g .. 64 g + 63 of the tile (accumulators
 //                 in registers), then all eight warps run the epilogue (bias/activation/residual/RoPE/SwiGLU -> global)
 //
+// With EWG (epilogue warpgroup, 512 threads: long-K launches without a stream-K tail, see gemm_dispatch) the epilogue has warpgroup 2 (warps 8..11)
+// to itself and the producer moves to warp 12 (warpgroup 3); setmaxnreg gives the registers the producer warpgroup does
+// not need to the others (40 / 152 / 168).  A consumer warpgroup waits on `staging_empty`, stores its accumulators to the
+// staging tile, arrives on `staging_full` and starts the next tile's main loop at once; the epilogue warpgroup waits on
+// `staging_full`, runs the same epilogue code over both column halves of its rows and arrives on `staging_empty`.  The
+// tensor cores then stall only while the accumulators are stored, not for the whole epilogue.
+//
 // Tile = 128 (M) x BN (N) x 64 (K) per stage, BN in {32, 64, 128}; wgmma shape 64 x BN x 16.  The fp32 accumulators pass
 // through a shared-memory staging tile so that each epilogue thread owns one output row (32 consecutive columns per chunk,
 // 64 B contiguous stores); the producer keeps filling the ring for the next tile meanwhile.  One CTA per SM, static
@@ -65,6 +72,15 @@ constexpr uint32_t kABytes = kBlockM * kBlockK * 2;  // 16 KiB per stage
 constexpr int kMaxBN = 128;
 constexpr int kGemmThreads = 288;  // 2 consumer warpgroups + 1 producer warp
 constexpr int kProducerWarp = 8;
+constexpr int kGemmThreadsEwg = 512;  // EWG: 2 consumer warpgroups + the epilogue warpgroup + the producer warpgroup
+constexpr int kProducerWarpEwg = 12;
+// Shortest K (in 64-deep k-blocks) launched with the epilogue warpgroup.  Below it the main loop is too short to hide the
+// epilogue of one warpgroup (which covers every column of its rows), and the eight consumer warps sharing the epilogue
+// may win.  One run of tools/bench_gemm_schedule.py with the epilogue warpgroup forced at every K (an H100 80GB HBM3 at a
+// 400 W limit, power-capped, fp16; its raw lines were not kept) had 8 and 16 k-blocks (Whisper, CLIP) 2-23 % slower with
+// it and 32 or more 6-13 % faster.  That card's clock moved between 435 and 1470 MHz, so the short-K losses are weak
+// evidence: the threshold keeps the old path where the new one was not shown to win.
+constexpr int kEwgMinKBlocks = 32;
 
 __host__ __device__ constexpr int gemm_stages(int BN) {
   // ring + fp32 staging tile within the 227 KiB an sm_90 block may use
@@ -319,11 +335,287 @@ constexpr bool epi_chunks_partition_tile() {
 
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
+// alpha times the per-row scale of output row `row` (row_scale, or the RMSNorm statistic derived from rs_sumsq)
+__device__ __forceinline__ float epi_row_scale(const GemmKParams& p, const TileCoord& t, int row) {
+  const bool row_ok = row < p.M;
+  float rs = 1.0f;
+  if (p.row_scale != nullptr && row_ok && !p.c_trans) rs = p.row_scale[static_cast<long long>(t.b) * p.M + row];
+  if (p.rs_sumsq != nullptr && row_ok) {
+    // RMSNorm statistic of this A row from the partial sums the PRODUCING GEMM's epilogue left behind (fixed summation
+    // order: deterministic)
+    const float4* sp = reinterpret_cast<const float4*>(p.rs_sumsq + static_cast<long long>(row) * p.rs_parts);
+    float ssum = 0.f;
+    for (int j = 0; j < p.rs_parts / 4; ++j) {
+      const float4 f = __ldg(sp + j);
+      ssum += (f.x + f.y) + (f.z + f.w);
+    }
+    rs = rsqrtf(ssum / static_cast<float>(p.K) + p.rs_eps);
+  }
+  return rs * p.alpha;
+}
+
+// Epilogue of one work unit for one epilogue row (q * 32 + lane of the tile) and one column half: reads the staged fp32
+// accumulators of that row (srow), then hands them to the tile's finisher (contributor piece) or adds the contributors'
+// partials and writes the outputs.  `wi` (0..7) is the stream-K flag / workspace lane of the (q, half) pair; `rs` is
+// epi_row_scale() (unused by a contributor piece).
+template <int BN, int EPI>
+__device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, const TileCoord& t, const GemmWork& wk, const float* srow,
+                                              float rs, int q, int lane, int half, int wi, int worker, int n_workers) {
+  const int n_out_total = (EPI == MM_EPI_SWIGLU) ? p.N / 2 : p.N;
+  const int row = t.m_blk * kBlockM + q * 32 + lane;
+  const bool row_ok = row < p.M;
+  if (wk.role == 1) {
+    // ---- stream-K contributor: hand the raw fp32 partial accumulator of this K-range to the tile's finisher.
+    // Slot layout [32-col chunk][4-col group 0..7][row 0..127][4 floats]: every warp store / load instruction moves
+    // 512 contiguous bytes; warp (q, half) writes exactly the chunks the finisher's warp (q, half) reads
+    // (epi_chunk), so the hand-over is per warp.
+    float* slot = p.sk_ws + static_cast<long long>(worker) * (kBlockM * BN);
+#pragma unroll 1
+    for (int j = 0; j < epi_chunk_count<BN, EPI>(); ++j) {
+      const int c = epi_chunk<BN, EPI>(half, j);
+      if (c < 0) continue;
+      uint32_t r[32];
+      stage_ld32(srow + c * 32, r);
+      float4* dst = reinterpret_cast<float4*>(slot) + static_cast<long long>(c) * 8 * kBlockM + q * 32 + lane;
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+        dst[i * kBlockM] = make_float4(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]), __uint_as_float(r[4 * i + 2]),
+                             __uint_as_float(r[4 * i + 3]));
+    }
+    __threadfence();
+    __syncwarp();
+    if (lane == 0) st_release_gpu(p.sk_flags + worker * 8 + wi, 1);
+    return;
+  }
+  // stream-K finisher: r[] += the contributors' partials of accumulator columns col_off .. col_off + 31 (fixed
+  // order: deterministic); a no-op for ordinary tiles (warp-uniform branch)
+  // (a CTA whose share of the tail is empty — more CTAs than tail k-blocks — has no piece and is skipped)
+  const unsigned sk_units = static_cast<unsigned>(p.sk_tiles) * p.num_k;
+  auto sk_has = [&](int sidx) {
+    return static_cast<unsigned>(sidx) * sk_units / n_workers < static_cast<unsigned>(sidx + 1) * sk_units / n_workers;
+  };
+  auto sk_add = [&](uint32_t (&r)[32], int col_off) {
+    if (wk.nc == 0) return;
+    const int c = col_off >> 5;
+    for (int sidx = wk.c0; sidx < wk.c0 + wk.nc; ++sidx) {
+      if (!sk_has(sidx)) continue;
+      const float4* src = reinterpret_cast<const float4*>(p.sk_ws + static_cast<long long>(sidx) * (kBlockM * BN)) +
+                          static_cast<long long>(c) * 8 * kBlockM + q * 32 + lane;
+      float4 fv[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) fv[i] = __ldcg(src + i * kBlockM);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float4 f = fv[i];
+        r[4 * i] = __float_as_uint(__uint_as_float(r[4 * i]) + f.x);
+        r[4 * i + 1] = __float_as_uint(__uint_as_float(r[4 * i + 1]) + f.y);
+        r[4 * i + 2] = __float_as_uint(__uint_as_float(r[4 * i + 2]) + f.z);
+        r[4 * i + 3] = __float_as_uint(__uint_as_float(r[4 * i + 3]) + f.w);
+      }
+    }
+  };
+  if (wk.nc > 0) {  // wait for this warp's share of every contributor's partial
+    if (lane == 0)
+      for (int sidx = wk.c0; sidx < wk.c0 + wk.nc; ++sidx)
+        if (sk_has(sidx)) {
+          unsigned spins = 0;
+          while (ld_acquire_gpu(p.sk_flags + sidx * 8 + wi) == 0) {
+            __nanosleep(64);
+            if (++spins > (1u << 25)) asm volatile("trap;");  // seconds: a scheduling bug must fail, never hang
+          }
+        }
+    __syncwarp();
+  }
+  char* crow = reinterpret_cast<char*>(p.C) +
+               (static_cast<long long>(t.b_lo) * p.c_bs + static_cast<long long>(t.b_hi) * p.c_bs2 +
+                static_cast<long long>(row) * p.ldc) * (p.c_fp32 ? 4 : 2);
+  if constexpr (EPI == MM_EPI_STD) {
+    if (p.c_trans) {
+      // "swap-AB" launches (few activation rows, many weight rows): the tile's rows are OUTPUT FEATURES (weights ride
+      // the 128-row A operand so every MMA row is useful) and its columns are the activation rows.  C / residual are
+      // addressed transposed, bias is per tile row, row_scale per tile column.  Outputs are tiny: scalar stores.
+      const float bias_r = (p.bias != nullptr && row_ok) ? aux_ld(p.bias, row, p.aux_f16) : 0.f;
+#pragma unroll 1
+      for (int j = 0; j < epi_chunk_count<BN, EPI>(); ++j) {
+        const int c = epi_chunk<BN, EPI>(half, j);
+        if (c < 0) continue;
+        uint32_t r[32];
+        stage_ld32(srow + c * 32, r);
+        sk_add(r, c * 32);
+        const int col0 = t.n_blk * BN + c * 32;
+        if (col0 >= p.N || !row_ok) continue;
+        float v[32];
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const int col = col0 + i;
+          float cs = p.alpha;
+          if (p.row_scale != nullptr && col < p.N) cs *= p.row_scale[col];
+          v[i] = __uint_as_float(r[i]) * cs + bias_r;
+        }
+        if (p.act != MM_ACT_NONE) apply_act32(v, p.act);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const int col = col0 + i;
+          if (col < p.N) {
+            float o = v[i];
+            if (p.residual != nullptr) o += aux_ld(p.residual, static_cast<long long>(col) * p.ldr + row, p.aux_f16);
+            if (p.c_fp32)
+              reinterpret_cast<float*>(p.C)[static_cast<long long>(col) * p.ldc + row] = o;
+            else if (p.c_fp16)
+              reinterpret_cast<__half*>(p.C)[static_cast<long long>(col) * p.ldc + row] = __float2half_rn(o);
+            else
+              reinterpret_cast<bf16*>(p.C)[static_cast<long long>(col) * p.ldc + row] = __float2bfloat16(o);
+          }
+        }
+      }
+    } else {
+    const bf16* bias = p.bias ? p.bias + static_cast<long long>(t.b_lo) * p.bias_bs : nullptr;
+    const bf16* rrow = nullptr;
+    if (p.residual != nullptr && row_ok) {
+      const int rr = p.res_row_mod > 0 ? row % p.res_row_mod : row;
+      rrow = p.residual + static_cast<long long>(t.b_lo) * p.r_bs + static_cast<long long>(t.b_hi) * p.r_bs2 +
+             static_cast<long long>(rr) * p.ldr;
+    }
+#pragma unroll 1
+    for (int j = 0; j < epi_chunk_count<BN, EPI>(); ++j) {
+      const int c = epi_chunk<BN, EPI>(half, j);
+      if (c < 0) continue;
+      uint32_t r[32];
+      stage_ld32(srow + c * 32, r);
+      sk_add(r, c * 32);
+      const int col0 = t.n_blk * BN + c * 32;
+      if (col0 >= p.N) continue;  // warp-uniform
+      float v[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]) * rs;
+      const bool full = p.vec_ok && (col0 + 32 <= p.N);
+      if (p.bias_rs != nullptr || p.bias2 != nullptr) {
+        // row-scaled bias terms (value-side biases of the absorbed alignment attention); narrow GEMMs only
+        const long long ri = static_cast<long long>(t.b) * p.M + row;
+        const float s1 = (p.bias_rs != nullptr && row_ok) ? p.bias_rs[ri] : 1.0f;
+        const float s2 = (p.bias2_rs != nullptr && row_ok) ? p.bias2_rs[ri] : 1.0f;
+        const bf16* b2 = p.bias2 ? p.bias2 + static_cast<long long>(t.b_lo) * p.bias_bs : nullptr;
+#pragma unroll
+        for (int i = 0; i < 32; ++i)
+          if (col0 + i < p.N) {
+            if (bias != nullptr) v[i] = fmaf(s1, aux_ld(bias, col0 + i, p.aux_f16), v[i]);
+            if (b2 != nullptr) v[i] = fmaf(s2, aux_ld(b2, col0 + i, p.aux_f16), v[i]);
+          }
+      } else if (bias != nullptr) {
+        if (full) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i)
+            aux_add8(v + 8 * i, __ldg(reinterpret_cast<const uint4*>(bias + col0) + i), p.aux_f16);
+        } else {
+#pragma unroll
+          for (int i = 0; i < 32; ++i)
+            if (col0 + i < p.N) v[i] += aux_ld(bias, col0 + i, p.aux_f16);
+        }
+      }
+      if (p.act != MM_ACT_NONE) apply_act32(v, p.act);
+      if (rrow != nullptr) {
+        if (full) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) aux_add8(v + 8 * i, *(reinterpret_cast<const uint4*>(rrow + col0) + i), p.aux_f16);
+        } else {
+#pragma unroll
+          for (int i = 0; i < 32; ++i)
+            if (col0 + i < p.N) v[i] += aux_ld(rrow, col0 + i, p.aux_f16);
+        }
+      }
+      if (row_ok) store_row32(p, crow, col0, n_out_total, v);
+      if (p.sumsq_out != nullptr && row_ok) {
+        // sum of squares of the values AS STORED (rounded to the output format), for the next RMSNorm
+        float ss = 0.f;
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          const float r = p.c_fp16 ? __half2float(__float2half_rn(v[i])) : __bfloat162float(__float2bfloat16(v[i]));
+          ss = fmaf(r, r, ss);
+        }
+        p.sumsq_out[static_cast<long long>(row) * p.sumsq_parts + (col0 >> 5)] = ss;
+      }
+    }
+    }  // !c_trans
+  } else if constexpr (EPI == MM_EPI_SWIGLU) {
+#pragma unroll 1
+    for (int j = 0; j < epi_chunk_count<BN, EPI>(); j += 2) {
+      const int cg = epi_chunk<BN, EPI>(half, j), cu = epi_chunk<BN, EPI>(half, j + 1);  // [32 gate | 32 up]
+      uint32_t g[32], u[32];
+      stage_ld32(srow + cg * 32, g);
+      stage_ld32(srow + cu * 32, u);
+      sk_add(g, cg * 32);
+      sk_add(u, cu * 32);
+      const int col_in = t.n_blk * BN + cg * 32;
+      if (col_in >= p.N) continue;
+      float v[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const float gg = __uint_as_float(g[i]) * rs;
+        const float uu = __uint_as_float(u[i]) * rs;
+        v[i] = gg * sigmoid_fast(gg) * uu;
+      }
+      if (row_ok) store_row32(p, crow, col_in / 2, n_out_total, v);
+    }
+  } else {  // MM_EPI_ROPE, head_dim 128: pairs (i, i + 64) within each head
+    const int pos = (row_ok ? (row % p.rope_T) : 0) + (p.rope_pos != nullptr ? __ldg(p.rope_pos) : 0);
+    const float* cs = p.rope_cos + static_cast<long long>(pos) * 64;
+    const float* sn = p.rope_sin + static_cast<long long>(pos) * 64;
+#pragma unroll 1
+    for (int j = 0; j < epi_chunk_count<BN, EPI>(); j += 2) {
+      {
+        const int c1 = epi_chunk<BN, EPI>(half, j), c2 = epi_chunk<BN, EPI>(half, j + 1);  // columns i and i + 64
+        const int hc = c1 & 1;  // which 32 of the head's first 64 columns
+        uint32_t x1[32], x2[32];
+        stage_ld32(srow + c1 * 32, x1);
+        stage_ld32(srow + c2 * 32, x2);
+        sk_add(x1, c1 * 32);
+        sk_add(x2, c2 * 32);
+        const int col1 = t.n_blk * BN + c1 * 32;
+        if (col1 >= p.N) continue;
+        float o1[32], o2[32];
+        if (col1 < p.rope_cols) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const float4 c4 = __ldg(reinterpret_cast<const float4*>(cs + hc * 32) + i);
+            const float4 s4 = __ldg(reinterpret_cast<const float4*>(sn + hc * 32) + i);
+            const float cc[4] = {c4.x, c4.y, c4.z, c4.w};
+            const float ss[4] = {s4.x, s4.y, s4.z, s4.w};
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+              const float a = __uint_as_float(x1[4 * i + j]) * rs;
+              const float b = __uint_as_float(x2[4 * i + j]) * rs;
+              o1[4 * i + j] = a * cc[j] - b * ss[j];
+              o2[4 * i + j] = b * cc[j] + a * ss[j];
+            }
+          }
+        } else {
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            o1[i] = __uint_as_float(x1[i]) * rs;
+            o2[i] = __uint_as_float(x2[i]) * rs;
+          }
+        }
+        if (row_ok) {
+          store_row32(p, crow, col1, n_out_total, o1);
+          store_row32(p, crow, col1 + 64, n_out_total, o2);
+        }
+      }
+    }
+  }
+  if (wk.nc > 0) {  // partials consumed: re-arm this warp's flags for the next launch (stream order separates launches)
+    __syncwarp();
+    if (lane == 0)
+      for (int sidx = wk.c0; sidx < wk.c0 + wk.nc; ++sidx)
+        if (sk_has(sidx)) p.sk_flags[sidx * 8 + wi] = 0;
+  }
+}
+
 // A_MN = true: A is given as [K][M] with M contiguous (the transpose of a row-major [tokens][features] activation): the
 // weight-gradient GEMM dW = dY^T X reads dY and X exactly as the forward pass wrote them, no transpose copies.
 // B_MN = true: B is given as [K][N] with N contiguous.  F16: IEEE half operands, else bf16.
-template <int BN, int EPI, bool B_MN, bool A_MN, bool F16>
-__global__ void __launch_bounds__(kGemmThreads, 1)
+// EWG = true: the epilogue runs in its own warpgroup (see the file comment) while the consumers start the next tile.
+template <int BN, int EPI, bool B_MN, bool A_MN, bool F16, bool EWG>
+__global__ void __launch_bounds__(EWG ? kGemmThreadsEwg : kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const GemmKParams p) {
   static_assert(BN == 32 || BN == 64 || BN == 128, "wgmma tile width");
@@ -339,7 +631,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   float* sC = reinterpret_cast<float*>(sB + STAGES * B_BYTES);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(sC + kBlockM * LDS);
   uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* staging_full = empty_bar + STAGES;  // EWG: the consumers have written a tile's accumulators to sC
+  uint64_t* staging_empty = staging_full + 1;   // EWG: the epilogue warpgroup is done with sC
 
+  constexpr int kProducer = EWG ? kProducerWarpEwg : kProducerWarp;
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int worker = static_cast<int>(blockIdx.x);
@@ -347,12 +642,16 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int m_units = p.m_tiles;
   const int total_tiles = p.batch * p.batch2 * m_units * p.n_tiles;
 
-  if (warp == kProducerWarp && elect_one()) {
+  if (warp == kProducer && elect_one()) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
+    }
+    if constexpr (EWG) {
+      mbar_init(staging_full, 256);  // every consumer thread, after its accumulator stores
+      mbar_init(staging_empty, 128);  // every epilogue thread, after its last staging read
     }
     fence_mbar_init();
   }
@@ -361,9 +660,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   griddep_launch();
   griddep_wait();
 
-  if (warp == kProducerWarp) {
+  if (warp >= kProducer) {
     // ------------------------------------------------------------------ TMA producer
-    if (elect_one()) {
+    if constexpr (EWG) setmaxnreg_dec<40>();
+    if (warp == kProducer && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
       GemmWork wk;
@@ -400,13 +700,28 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     return;
   }
 
-  // -------------------------------------------------------------------- consumers: main loop, then epilogue
-  const int wg = warp >> 2;
-  const int q = warp & 3;     // the epilogue rows of this warp: q * 32 + lane
-  const int half = warp >> 2;  // which half of the tile's columns this warp's epilogue handles
-  const int n_out_total = (EPI == MM_EPI_SWIGLU) ? p.N / 2 : p.N;
-  const int wi = warp;  // 0..7: this warp's private flag / workspace lane of the stream-K hand-over
+  const int q = warp & 3;  // the epilogue rows of this warp: q * 32 + lane
   const float* srow = sC + (q * 32 + lane) * LDS;
+  if (EWG && warp >= 8) {
+    // ------------------------------------------------------------------ epilogue warpgroup: every column of its rows
+    if constexpr (EWG) setmaxnreg_inc<168>();
+    GemmWork wk;
+    // EWG launches have no stream-K tail (launch_gemm refuses one): every work unit is a whole tile (role 0), so the
+    // stream-K flag lane passed below is never used
+    for (int it = 0; gemm_work(p, worker, n_workers, total_tiles, it, wk); ++it) {
+      const TileCoord t = tile_coord(wk.tile, p, m_units);
+      // the row statistic's L2 reads are issued before the wait: they overlap the tile's main loop
+      const float rs = epi_row_scale(p, t, t.m_blk * kBlockM + q * 32 + lane);
+      mbar_wait(staging_full, it & 1);
+      for (int half = 0; half < 2; ++half) gemm_epilogue<BN, EPI>(p, t, wk, srow, rs, q, lane, half, q + 4 * half, worker, n_workers);
+      mbar_arrive(staging_empty);
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers: main loop (then epilogue, EWG off)
+  if constexpr (EWG) setmaxnreg_inc<152>();
+  const int wg = warp >> 2;
   int stage = 0;
   uint32_t phase = 0;
   GemmWork wk;
@@ -446,7 +761,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
       // accumulators -> staging tile (the previous tile's epilogue must be done reading it)
-      consumer_sync();
+      if constexpr (EWG) mbar_wait(staging_empty, (it & 1) ^ 1);
+      else consumer_sync();
       const int r0 = wg * 64 + q * 16 + (lane >> 2);
       const int c0 = 2 * (lane & 3);
 #pragma unroll
@@ -454,271 +770,17 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         *reinterpret_cast<float2*>(sC + r0 * LDS + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
         *reinterpret_cast<float2*>(sC + (r0 + 8) * LDS + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       }
+      if constexpr (EWG) {
+        mbar_arrive(staging_full);
+        continue;  // straight on to the next tile's main loop
+      }
       consumer_sync();
     }
-    {  // epilogue of this work unit
-      const int row = t.m_blk * kBlockM + q * 32 + lane;
-      const bool row_ok = row < p.M;
-      if (wk.role == 1) {
-        // ---- stream-K contributor: hand the raw fp32 partial accumulator of this K-range to the tile's finisher.
-        // Slot layout [32-col chunk][4-col group 0..7][row 0..127][4 floats]: every warp store / load instruction moves
-        // 512 contiguous bytes; warp (q, half) writes exactly the chunks the finisher's warp (q, half) reads
-        // (epi_chunk), so the hand-over is per warp.
-        float* slot = p.sk_ws + static_cast<long long>(worker) * (kBlockM * BN);
-#pragma unroll 1
-        for (int j = 0; j < epi_chunk_count<BN, EPI>(); ++j) {
-          const int c = epi_chunk<BN, EPI>(half, j);
-          if (c < 0) continue;
-          uint32_t r[32];
-          stage_ld32(srow + c * 32, r);
-          float4* dst = reinterpret_cast<float4*>(slot) + static_cast<long long>(c) * 8 * kBlockM + q * 32 + lane;
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            dst[i * kBlockM] = make_float4(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]), __uint_as_float(r[4 * i + 2]),
-                                 __uint_as_float(r[4 * i + 3]));
-        }
-        __threadfence();
-        __syncwarp();
-        if (lane == 0) st_release_gpu(p.sk_flags + worker * 8 + wi, 1);
-        continue;
-      }
-      // stream-K finisher: r[] += the contributors' partials of accumulator columns col_off .. col_off + 31 (fixed
-      // order: deterministic); a no-op for ordinary tiles (warp-uniform branch)
-      // (a CTA whose share of the tail is empty — more CTAs than tail k-blocks — has no piece and is skipped)
-      const unsigned sk_units = static_cast<unsigned>(p.sk_tiles) * p.num_k;
-      auto sk_has = [&](int sidx) {
-        return static_cast<unsigned>(sidx) * sk_units / n_workers < static_cast<unsigned>(sidx + 1) * sk_units / n_workers;
-      };
-      auto sk_add = [&](uint32_t (&r)[32], int col_off) {
-        if (wk.nc == 0) return;
-        const int c = col_off >> 5;
-        for (int sidx = wk.c0; sidx < wk.c0 + wk.nc; ++sidx) {
-          if (!sk_has(sidx)) continue;
-          const float4* src = reinterpret_cast<const float4*>(p.sk_ws + static_cast<long long>(sidx) * (kBlockM * BN)) +
-                              static_cast<long long>(c) * 8 * kBlockM + q * 32 + lane;
-          float4 fv[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) fv[i] = __ldcg(src + i * kBlockM);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 f = fv[i];
-            r[4 * i] = __float_as_uint(__uint_as_float(r[4 * i]) + f.x);
-            r[4 * i + 1] = __float_as_uint(__uint_as_float(r[4 * i + 1]) + f.y);
-            r[4 * i + 2] = __float_as_uint(__uint_as_float(r[4 * i + 2]) + f.z);
-            r[4 * i + 3] = __float_as_uint(__uint_as_float(r[4 * i + 3]) + f.w);
-          }
-        }
-      };
-      if (wk.nc > 0) {  // wait for this warp's share of every contributor's partial
-        if (lane == 0)
-          for (int sidx = wk.c0; sidx < wk.c0 + wk.nc; ++sidx)
-            if (sk_has(sidx)) {
-              unsigned spins = 0;
-              while (ld_acquire_gpu(p.sk_flags + sidx * 8 + wi) == 0) {
-                __nanosleep(64);
-                if (++spins > (1u << 25)) asm volatile("trap;");  // seconds: a scheduling bug must fail, never hang
-              }
-            }
-        __syncwarp();
-      }
-      char* crow = reinterpret_cast<char*>(p.C) +
-                   (static_cast<long long>(t.b_lo) * p.c_bs + static_cast<long long>(t.b_hi) * p.c_bs2 +
-                    static_cast<long long>(row) * p.ldc) * (p.c_fp32 ? 4 : 2);
-      float rs = 1.0f;
-      if (p.row_scale != nullptr && row_ok && !p.c_trans) rs = p.row_scale[static_cast<long long>(t.b) * p.M + row];
-      if (p.rs_sumsq != nullptr && row_ok) {
-        // RMSNorm statistic of this A row from the partial sums the PRODUCING GEMM's epilogue left behind (fixed summation
-        // order: deterministic); done while this tile's MMAs are still running
-        const float4* sp = reinterpret_cast<const float4*>(p.rs_sumsq + static_cast<long long>(row) * p.rs_parts);
-        float ssum = 0.f;
-        for (int j = 0; j < p.rs_parts / 4; ++j) {
-          const float4 f = __ldg(sp + j);
-          ssum += (f.x + f.y) + (f.z + f.w);
-        }
-        rs = rsqrtf(ssum / static_cast<float>(p.K) + p.rs_eps);
-      }
-      rs *= p.alpha;
-
-      if constexpr (EPI == MM_EPI_STD) {
-        if (p.c_trans) {
-          // "swap-AB" launches (few activation rows, many weight rows): the tile's rows are OUTPUT FEATURES (weights ride
-          // the 128-row A operand so every MMA row is useful) and its columns are the activation rows.  C / residual are
-          // addressed transposed, bias is per tile row, row_scale per tile column.  Outputs are tiny: scalar stores.
-          const float bias_r = (p.bias != nullptr && row_ok) ? aux_ld(p.bias, row, p.aux_f16) : 0.f;
-#pragma unroll 1
-          for (int j = 0; j < epi_chunk_count<BN, EPI>(); ++j) {
-            const int c = epi_chunk<BN, EPI>(half, j);
-            if (c < 0) continue;
-            uint32_t r[32];
-            stage_ld32(srow + c * 32, r);
-            sk_add(r, c * 32);
-            const int col0 = t.n_blk * BN + c * 32;
-            if (col0 >= p.N || !row_ok) continue;
-            float v[32];
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const int col = col0 + i;
-              float cs = p.alpha;
-              if (p.row_scale != nullptr && col < p.N) cs *= p.row_scale[col];
-              v[i] = __uint_as_float(r[i]) * cs + bias_r;
-            }
-            if (p.act != MM_ACT_NONE) apply_act32(v, p.act);
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const int col = col0 + i;
-              if (col < p.N) {
-                float o = v[i];
-                if (p.residual != nullptr) o += aux_ld(p.residual, static_cast<long long>(col) * p.ldr + row, p.aux_f16);
-                if (p.c_fp32)
-                  reinterpret_cast<float*>(p.C)[static_cast<long long>(col) * p.ldc + row] = o;
-                else if (p.c_fp16)
-                  reinterpret_cast<__half*>(p.C)[static_cast<long long>(col) * p.ldc + row] = __float2half_rn(o);
-                else
-                  reinterpret_cast<bf16*>(p.C)[static_cast<long long>(col) * p.ldc + row] = __float2bfloat16(o);
-              }
-            }
-          }
-        } else {
-        const bf16* bias = p.bias ? p.bias + static_cast<long long>(t.b_lo) * p.bias_bs : nullptr;
-        const bf16* rrow = nullptr;
-        if (p.residual != nullptr && row_ok) {
-          const int rr = p.res_row_mod > 0 ? row % p.res_row_mod : row;
-          rrow = p.residual + static_cast<long long>(t.b_lo) * p.r_bs + static_cast<long long>(t.b_hi) * p.r_bs2 +
-                 static_cast<long long>(rr) * p.ldr;
-        }
-#pragma unroll 1
-        for (int j = 0; j < epi_chunk_count<BN, EPI>(); ++j) {
-          const int c = epi_chunk<BN, EPI>(half, j);
-          if (c < 0) continue;
-          uint32_t r[32];
-          stage_ld32(srow + c * 32, r);
-          sk_add(r, c * 32);
-          const int col0 = t.n_blk * BN + c * 32;
-          if (col0 >= p.N) continue;  // warp-uniform
-          float v[32];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]) * rs;
-          const bool full = p.vec_ok && (col0 + 32 <= p.N);
-          if (p.bias_rs != nullptr || p.bias2 != nullptr) {
-            // row-scaled bias terms (value-side biases of the absorbed alignment attention); narrow GEMMs only
-            const long long ri = static_cast<long long>(t.b) * p.M + row;
-            const float s1 = (p.bias_rs != nullptr && row_ok) ? p.bias_rs[ri] : 1.0f;
-            const float s2 = (p.bias2_rs != nullptr && row_ok) ? p.bias2_rs[ri] : 1.0f;
-            const bf16* b2 = p.bias2 ? p.bias2 + static_cast<long long>(t.b_lo) * p.bias_bs : nullptr;
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (col0 + i < p.N) {
-                if (bias != nullptr) v[i] = fmaf(s1, aux_ld(bias, col0 + i, p.aux_f16), v[i]);
-                if (b2 != nullptr) v[i] = fmaf(s2, aux_ld(b2, col0 + i, p.aux_f16), v[i]);
-              }
-          } else if (bias != nullptr) {
-            if (full) {
-#pragma unroll
-              for (int i = 0; i < 4; ++i)
-                aux_add8(v + 8 * i, __ldg(reinterpret_cast<const uint4*>(bias + col0) + i), p.aux_f16);
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i)
-                if (col0 + i < p.N) v[i] += aux_ld(bias, col0 + i, p.aux_f16);
-            }
-          }
-          if (p.act != MM_ACT_NONE) apply_act32(v, p.act);
-          if (rrow != nullptr) {
-            if (full) {
-#pragma unroll
-              for (int i = 0; i < 4; ++i) aux_add8(v + 8 * i, *(reinterpret_cast<const uint4*>(rrow + col0) + i), p.aux_f16);
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i)
-                if (col0 + i < p.N) v[i] += aux_ld(rrow, col0 + i, p.aux_f16);
-            }
-          }
-          if (row_ok) store_row32(p, crow, col0, n_out_total, v);
-          if (p.sumsq_out != nullptr && row_ok) {
-            // sum of squares of the values AS STORED (rounded to the output format), for the next RMSNorm
-            float ss = 0.f;
-#pragma unroll
-            for (int i = 0; i < 32; ++i) {
-              const float r = p.c_fp16 ? __half2float(__float2half_rn(v[i])) : __bfloat162float(__float2bfloat16(v[i]));
-              ss = fmaf(r, r, ss);
-            }
-            p.sumsq_out[static_cast<long long>(row) * p.sumsq_parts + (col0 >> 5)] = ss;
-          }
-        }
-        }  // !c_trans
-      } else if constexpr (EPI == MM_EPI_SWIGLU) {
-#pragma unroll 1
-        for (int j = 0; j < epi_chunk_count<BN, EPI>(); j += 2) {
-          const int cg = epi_chunk<BN, EPI>(half, j), cu = epi_chunk<BN, EPI>(half, j + 1);  // [32 gate | 32 up]
-          uint32_t g[32], u[32];
-          stage_ld32(srow + cg * 32, g);
-          stage_ld32(srow + cu * 32, u);
-          sk_add(g, cg * 32);
-          sk_add(u, cu * 32);
-          const int col_in = t.n_blk * BN + cg * 32;
-          if (col_in >= p.N) continue;
-          float v[32];
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float gg = __uint_as_float(g[i]) * rs;
-            const float uu = __uint_as_float(u[i]) * rs;
-            v[i] = gg * sigmoid_fast(gg) * uu;
-          }
-          if (row_ok) store_row32(p, crow, col_in / 2, n_out_total, v);
-        }
-      } else {  // MM_EPI_ROPE, head_dim 128: pairs (i, i + 64) within each head
-        const int pos = (row_ok ? (row % p.rope_T) : 0) + (p.rope_pos != nullptr ? __ldg(p.rope_pos) : 0);
-        const float* cs = p.rope_cos + static_cast<long long>(pos) * 64;
-        const float* sn = p.rope_sin + static_cast<long long>(pos) * 64;
-#pragma unroll 1
-        for (int j = 0; j < epi_chunk_count<BN, EPI>(); j += 2) {
-          {
-            const int c1 = epi_chunk<BN, EPI>(half, j), c2 = epi_chunk<BN, EPI>(half, j + 1);  // columns i and i + 64
-            const int hc = c1 & 1;  // which 32 of the head's first 64 columns
-            uint32_t x1[32], x2[32];
-            stage_ld32(srow + c1 * 32, x1);
-            stage_ld32(srow + c2 * 32, x2);
-            sk_add(x1, c1 * 32);
-            sk_add(x2, c2 * 32);
-            const int col1 = t.n_blk * BN + c1 * 32;
-            if (col1 >= p.N) continue;
-            float o1[32], o2[32];
-            if (col1 < p.rope_cols) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) {
-                const float4 c4 = __ldg(reinterpret_cast<const float4*>(cs + hc * 32) + i);
-                const float4 s4 = __ldg(reinterpret_cast<const float4*>(sn + hc * 32) + i);
-                const float cc[4] = {c4.x, c4.y, c4.z, c4.w};
-                const float ss[4] = {s4.x, s4.y, s4.z, s4.w};
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                  const float a = __uint_as_float(x1[4 * i + j]) * rs;
-                  const float b = __uint_as_float(x2[4 * i + j]) * rs;
-                  o1[4 * i + j] = a * cc[j] - b * ss[j];
-                  o2[4 * i + j] = b * cc[j] + a * ss[j];
-                }
-              }
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) {
-                o1[i] = __uint_as_float(x1[i]) * rs;
-                o2[i] = __uint_as_float(x2[i]) * rs;
-              }
-            }
-            if (row_ok) {
-              store_row32(p, crow, col1, n_out_total, o1);
-              store_row32(p, crow, col1 + 64, n_out_total, o2);
-            }
-          }
-        }
-      }
-      if (wk.nc > 0) {  // partials consumed: re-arm this warp's flags for the next launch (stream order separates launches)
-        __syncwarp();
-        if (lane == 0)
-          for (int sidx = wk.c0; sidx < wk.c0 + wk.nc; ++sidx)
-            if (sk_has(sidx)) p.sk_flags[sidx * 8 + wi] = 0;
-      }
-    }
+    // epilogue of this work unit: warp (q, half) handles column half `half` of rows q * 32 + lane; warp w owns the
+    // stream-K flag / workspace lane w
+    const int half = warp >> 2;
+    const float rs = wk.role == 1 ? 1.0f : epi_row_scale(p, t, t.m_blk * kBlockM + q * 32 + lane);
+    gemm_epilogue<BN, EPI>(p, t, wk, srow, rs, q, lane, half, warp, worker, n_workers);
   }
 }
 
@@ -774,15 +836,27 @@ static int& streamk_mode() {
   return mode;
 }
 
+// process-wide epilogue-overlap policy; initial value from MACAW_B200_GEMM_OVERLAP (default 1)
+static int& overlap_mode() {
+  static int mode = []() { const char* e = getenv("MACAW_B200_GEMM_OVERLAP"); const int v = e ? atoi(e) : 1; return v < 0 || v > 1 ? 1 : v; }();
+  return mode;
+}
+
 template <int BN, int EPI, bool B_MN, bool A_MN = false>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmKParams& p, bool f16, cudaStream_t st) {
-  static bool attr_set[2][kMaxDevices] = {};
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmKParams& p, bool f16, bool ewg,
+                       cudaStream_t st) {
+  if (ewg && p.sk_tiles != 0) {  // the epilogue warpgroup implements whole tiles only (no stream-K hand-over)
+    set_error("mm_gemm_fwd: the epilogue-warpgroup kernel takes no stream-K tail");
+    return 1;
+  }
+  static bool attr_set[2][2][kMaxDevices] = {};
   constexpr size_t smem = gemm_smem_bytes(BN);
-  auto kern = f16 ? gemm_bf16_kernel<BN, EPI, B_MN, A_MN, true> : gemm_bf16_kernel<BN, EPI, B_MN, A_MN, false>;
-  if (int rc = ensure_smem_attr(kern, smem, attr_set[f16 ? 1 : 0], "mm_gemm_fwd")) return rc;
+  auto kern = f16 ? (ewg ? gemm_bf16_kernel<BN, EPI, B_MN, A_MN, true, true> : gemm_bf16_kernel<BN, EPI, B_MN, A_MN, true, false>)
+                  : (ewg ? gemm_bf16_kernel<BN, EPI, B_MN, A_MN, false, true> : gemm_bf16_kernel<BN, EPI, B_MN, A_MN, false, false>);
+  if (int rc = ensure_smem_attr(kern, smem, attr_set[f16 ? 1 : 0][ewg ? 1 : 0], "mm_gemm_fwd")) return rc;
   const int total = p.batch * p.batch2 * p.m_tiles * p.n_tiles;
   const int grid = (total < num_sms() && p.sk_tiles == 0) ? total : num_sms();  // stream-K shares the tail over ALL SMs
-  cudaError_t e = launch_kernel(kern, dim3(grid), dim3(kGemmThreads), smem, st, 1, ta, tb, p);
+  cudaError_t e = launch_kernel(kern, dim3(grid), dim3(ewg ? kGemmThreadsEwg : kGemmThreads), smem, st, 1, ta, tb, p);
   if (e != cudaSuccess) {
     set_error("mm_gemm_fwd: launch failed: %s", cudaGetErrorString(e));
     return 2;
@@ -951,13 +1025,16 @@ static int32_t gemm_dispatch(const mm_gemm_args* a, void* stream, mm_gemm_schedu
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   const bool f16 = a->a_fp16 != 0;
+  // A stream-K launch keeps the consumer epilogue: the epilogue warpgroup handles whole tiles only (the tail's pieces of
+  // one or two k-blocks would leave it nothing to overlap).
+  const bool ewg = overlap_mode() == 1 && p.num_k >= kEwgMinKBlocks && p.sk_tiles == 0;
 
-#define MM_LAUNCH(BN_, EPI_, MN_) return launch_gemm<BN_, EPI_, MN_>(ta, tb, p, f16, st)
+#define MM_LAUNCH(BN_, EPI_, MN_) return launch_gemm<BN_, EPI_, MN_>(ta, tb, p, f16, ewg, st)
   if (a->epi == MM_EPI_ROPE) MM_LAUNCH(128, MM_EPI_ROPE, false);
   if (a->epi == MM_EPI_SWIGLU) MM_LAUNCH(128, MM_EPI_SWIGLU, false);
   if (a->a_mn_major) {
-    if (BN == 128) return launch_gemm<128, MM_EPI_STD, true, true>(ta, tb, p, f16, st);
-    return launch_gemm<64, MM_EPI_STD, true, true>(ta, tb, p, f16, st);
+    if (BN == 128) return launch_gemm<128, MM_EPI_STD, true, true>(ta, tb, p, f16, ewg, st);
+    return launch_gemm<64, MM_EPI_STD, true, true>(ta, tb, p, f16, ewg, st);
   }
   if (a->b_mn_major) {
     if (BN == 128) MM_LAUNCH(128, MM_EPI_STD, true);
@@ -979,6 +1056,12 @@ extern "C" int32_t mm_gemm_plan(const mm_gemm_args* a, mm_gemm_schedule* plan) {
 extern "C" int32_t mm_gemm_streamk_mode(int32_t mode) {
   const int prev = streamk_mode();
   if (mode >= 0 && mode <= 2) streamk_mode() = mode;
+  return prev;
+}
+
+extern "C" int32_t mm_gemm_overlap_mode(int32_t mode) {
+  const int prev = overlap_mode();
+  if (mode >= 0 && mode <= 1) overlap_mode() = mode;
   return prev;
 }
 

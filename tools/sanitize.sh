@@ -20,3 +20,12 @@ timeout 900 compute-sanitizer --tool memcheck --error-exitcode 9 --print-limit 5
 echo "memcheck (alignment backward kernels) rc=$?"
 timeout 600 compute-sanitizer --tool racecheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_align_backward_gpu.py -q -x -m gpu -k "(align_softmax_bwd and (V32000-R97-drop-extra or V519 or V4097)) or (align_dropout_fwd and (V32000-R97-0.1 or V519))" --timeout 550 --timeout-method=thread 2>&1 | tail -8
 echo "racecheck (alignment backward kernels) rc=$?"
+# GEMM epilogue-overlap modes: the staging hand-over between the consumer and epilogue warpgroups (staging_full /
+# staging_empty mbarriers on the shared staging tile).  Every selected bit-identity case launches the epilogue-warpgroup
+# kernel in mode 1 (the test asserts it); the batch-32 shapes are left out for time.
+timeout 900 compute-sanitizer --tool memcheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_gemm_overlap_gpu.py -q -x -m gpu -k "300x or 8x4096 or 2112x4096x4096 or dw- or keep_consumer or setter" --timeout 850 --timeout-method=thread 2>&1 | tail -8
+echo "memcheck (GEMM overlap modes) rc=$?"
+timeout 900 compute-sanitizer --tool racecheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_gemm_overlap_gpu.py -q -x -m gpu -k "bit_identical and (bias_gelu-300x1000x2120 or row_scale_alpha-2112x4096x4096)" --timeout 850 --timeout-method=thread 2>&1 | tail -8
+echo "racecheck (GEMM overlap modes) rc=$?"
+timeout 900 compute-sanitizer --tool synccheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_gemm_overlap_gpu.py -q -x -m gpu -k "bit_identical and (bias_gelu-300x1000x2120 or row_scale_alpha-2112x4096x4096)" --timeout 850 --timeout-method=thread 2>&1 | tail -8
+echo "synccheck (GEMM overlap modes) rc=$?"
