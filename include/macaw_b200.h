@@ -286,6 +286,20 @@ int32_t mm_align_ctx_fixup(void* ctx, int64_t ldc, const float* p_sum_real, cons
 int32_t mm_kv_append(const void* qkv, int64_t ld_qkv, int32_t B, int32_t T_new, int32_t E, void* cache, int32_t Tmax,
                      int32_t t0, const int32_t* t0_dev, void* stream); /* t0_dev != NULL overrides t0 with a device int */
 int32_t mm_argmax_rows(const void* logits, int64_t ld, int32_t rows, int32_t V, int64_t* out, void* stream);
+/* mm_sample_rows: the next token of HF generate's decoding step (reference modeling.py:959 -> llm.generate with
+ * llm.generation_config): RepetitionPenaltyLogitsProcessor -> TemperatureLogitsWarper -> TopKLogitsWarper ->
+ * TopPLogitsWarper -> softmax -> multinomial, in fp32 on the 16-bit logits (rows, V), row stride ld, V <= 49152.
+ * seen: rows x ceil(V/32) uint32 bitmap of the tokens generated so far (the penalty's input_ids); the emitted token's bit
+ * is set.  top_k 0 = off, top_p 1 = off.  Top-k keeps scores >= the k-th largest; top-p removes token i iff the kept
+ * mass of all tokens with probability <= p_i is <= 1 - top_p (HF's ascending cumsum rule with tied probabilities
+ * resolved together; the largest token always stays).  Draw: u = (w >> 8) * 2^-24, w = word 0 of
+ * philox4x32_10(key = *seed_dev, counter = (*step_dev, row, 16, 0)); the token is the first kept one, in id order,
+ * whose cumulative unnormalised mass exceeds u * Z.  do_sample = 0: greedy search on the penalised scores (argmax,
+ * lowest index on ties; temperature / top-k / top-p unused, seed_dev / step_dev may be NULL).  The result is a pure
+ * function of the inputs (no order-dependent arithmetic). */
+int32_t mm_sample_rows(const void* logits, int64_t ld, int32_t rows, int32_t V, uint32_t* seen, float repetition_penalty,
+                       float temperature, int32_t top_k, float top_p, int32_t do_sample, const uint64_t* seed_dev,
+                       const int32_t* step_dev, int64_t* out, void* stream);
 /* Thin-row companions of the swapped-operand decode GEMMs (mm_gemm_args.c_trans), whose epilogue cannot pair columns:
  * mm_rope_rows: in-place rotate-half RoPE (head_dim 128, apply_rotary_pos_emb modeling.py:83-91) on the first rot_cols
  * columns; position of row r = (*pos_dev if given) + r % rope_T.  mm_swiglu_rows: out[r, j] = silu(gate_j) * up_j from

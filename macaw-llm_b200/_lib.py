@@ -130,6 +130,7 @@ SIGNATURES = {
     "mm_thin_fused": (c_i32, [C.POINTER(ThinArgs), c_vp]),
     "mm_thin_reduce": (c_i32, [c_vp, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp]),
     "mm_argmax_rows": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_vp]),
+    "mm_sample_rows": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_f32, c_f32, c_i32, c_f32, c_i32, c_vp, c_vp, c_vp, c_vp]),
     "mm_rope_rows": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp]),
     "mm_swiglu_rows": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_i64, c_vp]),
     "mm_rmsnorm_bwd": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_vp]),

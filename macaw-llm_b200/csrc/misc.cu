@@ -4,6 +4,7 @@
 #include "common.cuh"
 #include <cuda_fp16.h>
 #include "ptx.cuh"
+#include "philox.cuh"
 #include "../../include/macaw_b200.h"
 
 namespace mm {
@@ -705,6 +706,231 @@ __global__ void __launch_bounds__(512) argmax_rows_kernel(const bf16* __restrict
   }
 }
 
+// ------------------------------------------------------------------------------------------------ sampled next token
+// HF's processor chain for do_sample (RepetitionPenalty -> Temperature -> TopK -> TopP -> softmax -> multinomial), one CTA
+// per row, the row's fp32 scores in shared memory.  Probability masses are unsigned 64-bit fixed point,
+// round(exp(s - max) * 2^40): integer sums do not depend on the order they are taken in, so the token is a pure function
+// of (logits, bitmap, parameters, seed, step).  A token with exp(s - max) < 2^-41 gets mass 0 (it is never drawn; HF
+// would draw it with probability < 2^-41).
+constexpr int kSampleThreads = 512;
+constexpr int kSampleMaxV = 49152;  // 192 KiB of fp32 scores
+
+// order-preserving map of fp32 onto uint32 (a > b <=> key(a) > key(b)) and its inverse
+__device__ __forceinline__ uint32_t ord_key(float f) {
+  const uint32_t u = __float_as_uint(f);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float ord_key_inv(uint32_t k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+__device__ __forceinline__ unsigned long long mass_fx(float e) { return __float2ull_rn(e * 1099511627776.f); }
+
+__device__ __forceinline__ unsigned long long warp_incl_scan(unsigned long long v, int lane) {
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long n = __shfl_up_sync(0xffffffffu, v, o);
+    if (lane >= o) v += n;
+  }
+  return v;
+}
+
+// Radix select, 8 bits per pass from the top.  Scans the 256 digits of each pass in descending (DESC) or ascending key
+// order and returns the key at which the running weight first reaches `need`:
+//   DESC, weight 1                   -> the need-th largest key (top-k threshold)
+//   ascending, weight mass_fx(score) -> the smallest key K with M(key <= K) >= need (top-p threshold)
+// Keys: ord_key(score) for DESC, the raw bits of the (non-negative) score otherwise.  Every thread returns the key.
+template <bool DESC>
+__device__ uint32_t radix_select(const float* s, int V, unsigned long long need, unsigned long long* hist,
+                                 uint32_t* sel_digit, unsigned long long* sel_need) {
+  const int tid = threadIdx.x, lane = tid & 31;
+  uint32_t prefix = 0, pmask = 0;
+  for (int shift = 24; shift >= 0; shift -= 8) {
+    for (int i = tid; i < 256; i += kSampleThreads) hist[i] = 0ull;
+    __syncthreads();
+    for (int c = tid; c < V; c += kSampleThreads) {
+      const float f = s[c];
+      const uint32_t k = DESC ? ord_key(f) : __float_as_uint(f);
+      const bool in = (k & pmask) == prefix;
+      const uint32_t d = (k >> shift) & 255u;
+      if (DESC) {  // counts: one atomic per group of lanes with the same digit (the first passes hit a few digits)
+        const uint32_t peers = __match_any_sync(__activemask(), in ? d : 256u);
+        if (in && lane == __ffs(peers) - 1) atomicAdd(&hist[d], static_cast<unsigned long long>(__popc(peers)));
+      } else if (in && f != 0.f) {  // masses; the tokens top-k removed carry none
+        atomicAdd(&hist[d], mass_fx(f));  // integer: the sum does not depend on the order
+      }
+    }
+    __syncthreads();
+    if (tid < 32) {
+      // lane l owns scan positions 8l .. 8l + 7
+      unsigned long long h[8], sum = 0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int pos = 8 * lane + j;
+        h[j] = hist[DESC ? 255 - pos : pos];
+        sum += h[j];
+      }
+      const unsigned long long incl = warp_incl_scan(sum, lane);
+      const uint32_t hit = __ballot_sync(0xffffffffu, incl >= need);
+      // need <= total weight by construction; `hit == 0` cannot happen, the last digit is the safe answer if it did
+      const int first = hit ? __ffs(hit) - 1 : 31;
+      if (lane == first) {
+        unsigned long long cum = incl - sum;
+        int d = 7;
+#pragma unroll
+        for (int j = 7; j >= 0; --j) {  // the lowest j with cum(<= j) >= need
+          unsigned long long c2 = cum;
+#pragma unroll
+          for (int i = 0; i < 8; ++i) c2 += i <= j ? h[i] : 0ull;
+          if (c2 >= need) d = j;
+        }
+        unsigned long long before = cum;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) before += i < d ? h[i] : 0ull;
+        const int pos = 8 * lane + d;
+        *sel_digit = static_cast<uint32_t>(DESC ? 255 - pos : pos);
+        *sel_need = need - before;
+      }
+    }
+    __syncthreads();
+    prefix |= *sel_digit << shift;
+    pmask |= 255u << shift;
+    need = *sel_need;
+    __syncthreads();  // the next pass rewrites sel_* and hist
+  }
+  return prefix;
+}
+
+template <bool F16>
+__global__ void __launch_bounds__(kSampleThreads) sample_rows_kernel(
+    const bf16* __restrict__ logits, long long ld, int V, uint32_t* __restrict__ seen, int words, float penalty,
+    float temperature, int top_k, float top_p, int do_sample, const unsigned long long* __restrict__ seed_dev,
+    const int* __restrict__ step_dev, long long* __restrict__ out) {
+  extern __shared__ float s[];  // [V] fp32 scores, then unnormalised probabilities (do_sample only)
+  __shared__ unsigned long long hist[256];
+  __shared__ unsigned long long wsum[kSampleThreads / 32];
+  __shared__ float sv[kSampleThreads / 32];
+  __shared__ int si[kSampleThreads / 32];
+  __shared__ uint32_t sel_digit;
+  __shared__ unsigned long long sel_need;
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5, nw = kSampleThreads / 32;
+  const bf16* x = logits + static_cast<long long>(blockIdx.x) * ld;
+  uint32_t* bits = seen + static_cast<long long>(blockIdx.x) * words;
+  const bool pen = penalty != 1.f;
+
+  // 1. penalty (RepetitionPenaltyLogitsProcessor) and temperature, fp32; argmax with the lowest index on ties
+  float best = -INFINITY;
+  int bi = 0x7fffffff;
+  for (int c = tid; c < V; c += kSampleThreads) {
+    float v = ldv<F16>(x[c]);
+    if (pen && ((bits[c >> 5] >> (c & 31)) & 1u)) v = v < 0.f ? __fmul_rn(v, penalty) : __fdiv_rn(v, penalty);
+    if (do_sample) {
+      v = __fdiv_rn(v, temperature);
+      s[c] = v;
+    }
+    if (v > best || (v == best && c < bi)) {
+      best = v;
+      bi = c;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ov > best || (ov == best && oi < bi)) {
+      best = ov;
+      bi = oi;
+    }
+  }
+  if (lane == 0) {
+    sv[w] = best;
+    si[w] = bi;
+  }
+  __syncthreads();
+  best = sv[0];
+  bi = si[0];
+  for (int i = 1; i < nw; ++i)
+    if (sv[i] > best || (sv[i] == best && si[i] < bi)) {
+      best = sv[i];
+      bi = si[i];
+    }
+  if (!do_sample) {  // greedy search on the penalised scores
+    if (tid == 0) {
+      out[blockIdx.x] = bi;
+      bits[bi >> 5] |= 1u << (bi & 31);
+    }
+    return;
+  }
+
+  // 2. top-k: keep every score >= the k-th largest (ties at the boundary kept, as torch.topk and `<` give)
+  float kth = -INFINITY;
+  if (top_k > 0 && top_k < V) kth = ord_key_inv(radix_select<true>(s, V, static_cast<unsigned long long>(top_k), hist,
+                                                                    &sel_digit, &sel_need));
+  // 3. unnormalised softmax of the kept scores; best (the largest score) is always kept
+  unsigned long long z = 0;
+  for (int c = tid; c < V; c += kSampleThreads) {
+    const float v = s[c];
+    const float e = v >= kth ? expf(v - best) : 0.f;
+    s[c] = e;
+    z += mass_fx(e);
+  }
+  // 4. top-p: remove token i iff M(<= p_i) <= 1 - top_p, M(<= p) = the kept mass of the tokens with probability <= p
+  if (top_p < 1.f) {
+    z = warp_incl_scan(z, lane);
+    __syncthreads();
+    if (lane == 31) wsum[w] = z;
+    __syncthreads();
+    z = 0;
+    for (int i = 0; i < nw; ++i) z += wsum[i];
+    unsigned long long limit = static_cast<unsigned long long>((1.0 - static_cast<double>(top_p)) * static_cast<double>(z));
+    if (limit >= z) limit = z - 1;  // the largest token always stays
+    const uint32_t kmin = radix_select<false>(s, V, limit + 1, hist, &sel_digit, &sel_need);
+    for (int c = tid; c < V; c += kSampleThreads)
+      if (__float_as_uint(s[c]) < kmin) s[c] = 0.f;
+  }
+  __syncthreads();
+
+  // 5. inverse-CDF draw in token-id order: the first token whose inclusive mass prefix exceeds u * Z,
+  //    u = (word0 >> 8) * 2^-24, word0 of philox(key = seed, counter = (step, row, SID_SAMPLE, 0))
+  const int seg = ((V + nw - 1) / nw + 31) & ~31;  // warp w scans tokens [w * seg, (w + 1) * seg)
+  const int c0 = w * seg, c1 = min(V, c0 + seg);
+  unsigned long long part = 0;
+  for (int c = c0 + lane; c < c1; c += 32) part += mass_fx(s[c]);
+  part = warp_incl_scan(part, lane);
+  if (lane == 31) wsum[w] = part;
+  __syncthreads();
+  unsigned long long tot = 0;
+  for (int i = 0; i < nw; ++i) tot += wsum[i];
+  const unsigned long long seed = *seed_dev;
+  uint32_t ctr[4] = {static_cast<uint32_t>(*step_dev), blockIdx.x, SID_SAMPLE, 0u};
+  philox4x32_10(ctr, static_cast<uint32_t>(seed), static_cast<uint32_t>(seed >> 32));
+  const unsigned long long r = ctr[0] >> 8;
+  // cum * 2^24 > r * Z  <=>  cum > floor(r * Z / 2^24); r * Z < 2^79, Z < 2^56
+  const unsigned long long tgt = (__umul64hi(r, tot) << 40) | ((r * tot) >> 24);
+  unsigned long long carry = 0;
+  int wt = nw - 1;
+  for (int i = 0; i < nw; ++i) {
+    if (carry + wsum[i] > tgt) {
+      wt = i;
+      break;
+    }
+    carry += wsum[i];
+  }
+  if (w != wt) return;
+  for (int base = c0; base < c1; base += 32) {
+    const int c = base + lane;
+    const unsigned long long cum = carry + warp_incl_scan(c < c1 ? mass_fx(s[c]) : 0ull, lane);
+    const uint32_t hit = __ballot_sync(0xffffffffu, cum > tgt && c < c1);
+    if (hit) {
+      if (lane == __ffs(hit) - 1) {
+        out[blockIdx.x] = c;
+        bits[c >> 5] |= 1u << (c & 31);
+      }
+      return;
+    }
+    carry = __shfl_sync(0xffffffffu, cum, 31);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ CE loss
 template <bool F16>
 __global__ void __launch_bounds__(512) ce_loss_kernel(const bf16* __restrict__ logits, const long long* __restrict__ labels,
@@ -955,6 +1181,29 @@ extern "C" int32_t mm_argmax_rows(const void* logits, int64_t ld, int32_t rows, 
   auto kern = act_f16() ? argmax_rows_kernel<true> : argmax_rows_kernel<false>;
   kern<<<rows, 512, 0, ST(stream)>>>((const bf16*)logits, ld, V, (long long*)out);
   return check_launch("mm_argmax_rows");
+}
+
+extern "C" int32_t mm_sample_rows(const void* logits, int64_t ld, int32_t rows, int32_t V, uint32_t* seen,
+                                  float repetition_penalty, float temperature, int32_t top_k, float top_p,
+                                  int32_t do_sample, const uint64_t* seed_dev, const int32_t* step_dev, int64_t* out,
+                                  void* stream) {
+  MM_REQUIRE(logits && seen && out && rows > 0 && V > 0 && ld >= V, "mm_sample_rows: bad arguments");
+  MM_REQUIRE(repetition_penalty > 0.f, "mm_sample_rows: repetition_penalty must be > 0, got %g", repetition_penalty);
+  if (do_sample) {
+    MM_REQUIRE(seed_dev && step_dev, "mm_sample_rows: sampling needs the device seed and step");
+    MM_REQUIRE(V <= kSampleMaxV, "mm_sample_rows: V = %d exceeds the shared-memory row of %d scores", V, kSampleMaxV);
+    MM_REQUIRE(temperature > 0.f, "mm_sample_rows: temperature must be > 0, got %g", temperature);
+    MM_REQUIRE(top_k >= 0 && top_p >= 0.f && top_p <= 1.f, "mm_sample_rows: top_k >= 0 and 0 <= top_p <= 1 needed");
+  }
+  static bool attr16[kMaxDevices], attr_bf[kMaxDevices];
+  const bool f16 = act_f16();
+  auto kern = f16 ? sample_rows_kernel<true> : sample_rows_kernel<false>;
+  const size_t smem = do_sample ? static_cast<size_t>(V) * sizeof(float) : 0;
+  if (int rc = ensure_smem_attr(kern, kSampleMaxV * sizeof(float), f16 ? attr16 : attr_bf, "mm_sample_rows")) return rc;
+  kern<<<rows, kSampleThreads, smem, ST(stream)>>>((const bf16*)logits, ld, V, seen, (V + 31) / 32, repetition_penalty,
+                                                   temperature, top_k, top_p, do_sample,
+                                                   (const unsigned long long*)seed_dev, step_dev, (long long*)out);
+  return check_launch("mm_sample_rows");
 }
 
 extern "C" int32_t mm_ce_loss(const void* logits, const int64_t* labels, int32_t B, int32_t T, int32_t V,

@@ -12,6 +12,10 @@
 
 namespace mm {
 
+// Stream id of the token sampler (mm_sample_rows).  The dropout sites use 1..4 (Engine.DROPOUT_SID); the sampler's
+// words come from counter = (step, row, SID_SAMPLE, 0) and never coincide with a dropout mask's.
+constexpr uint32_t SID_SAMPLE = 16u;
+
 __host__ __device__ inline void philox_round(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
   const uint64_t p0 = static_cast<uint64_t>(0xD2511F53u) * c[0];
   const uint64_t p1 = static_cast<uint64_t>(0xCD9E8D57u) * c[2];

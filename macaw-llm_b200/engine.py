@@ -707,14 +707,29 @@ class Engine:
         logits = self._lm_head(x)
         return logits.view(B, T, logits.shape[-1])
 
-    # ------------------------------------------------------------------------------------------------ greedy decoding
-    def generate(self, inputs: dict, max_new_tokens: int = 128, eos_token_id: int = 2, pad_token_id: int = 32006):
+    # ------------------------------------------------------------------------------------------------ decoding
+    def generate(self, inputs: dict, max_new_tokens: int = 128, eos_token_id: int = 2, pad_token_id: int = 32006, *,
+                 do_sample: bool = False, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0,
+                 repetition_penalty: float = 1.0, seed: Optional[int] = None):
         """The `inference` branch of MM_LLMs.forward (reference modeling.py:954-960):
         `llm.generate(inputs_embeds=..., max_new_tokens=128, eos_token_id=2, bos_token_id=1, pad_token_id=32006)` —
-        HF greedy search (no sampling, one beam) on the multimodal prefix.  As in the reference, NO attention mask is
-        handed to generate (padding positions are attended) and only the new tokens are returned.  Prefill runs the
-        normal forward kernels while filling a per-layer KV cache; every decode step is one pass of M = B GEMMs
-        (weight-streaming bound) and a Tq = 1 attention over the cache."""
+        HF generate with one beam on the multimodal prefix: greedy search, or multinomial sampling (do_sample) after
+        HF's temperature / top-k (0 = off) / top-p (1.0 = off) warpers; a repetition penalty over the generated tokens
+        applies in both modes.  As in the reference, NO attention mask is handed to generate (padding positions are
+        attended) and only the new tokens are returned.  Prefill runs the normal forward kernels while filling a
+        per-layer KV cache; every decode step is one pass of M = B GEMMs (weight-streaming bound) and a Tq = 1
+        attention over the cache.  `seed` (64-bit) fixes the draws; when None it is drawn from torch's default CPU
+        generator, so torch.manual_seed makes a call reproducible."""
+        do_sample = bool(do_sample)
+        sampler = do_sample or float(repetition_penalty) != 1.0
+        if not float(repetition_penalty) > 0.0:
+            raise ValueError(f"macaw_b200: repetition_penalty must be > 0, got {repetition_penalty}")
+        if do_sample and not (float(temperature) > 0.0 and int(top_k) >= 0 and 0.0 <= float(top_p) <= 1.0):
+            raise ValueError(f"macaw_b200: sampling needs temperature > 0, top_k >= 0 and 0 <= top_p <= 1; got "
+                             f"temperature={temperature}, top_k={top_k}, top_p={top_p}")
+        if do_sample and seed is None:
+            lo, hi = torch.randint(0, 2 ** 32, (2,), dtype=torch.int64).tolist()
+            seed = lo | (hi << 32)
         with torch.no_grad():
             embeds, _, _ = self.prepare_inputs({k: v for k, v in inputs.items() if k not in ("labels", "attention_mask")})
             ops.TAG = "llama"
@@ -731,7 +746,7 @@ class Engine:
             key = (B, t_max, str(dev))
             st = self._decode.get(key)
             if st is None or st["stamp"] != stamp:
-                st = dict(stamp=stamp, graph=None,
+                st = dict(stamp=stamp, graphs={},
                           cache=[torch.zeros((B, t_max, 2, E), device=dev, dtype=ADT()) for _ in range(n_layers)],
                           finished=torch.zeros((B,), device=dev, dtype=torch.bool),
                           pos_dev=torch.zeros((2,), device=dev, dtype=torch.int32),
@@ -744,7 +759,31 @@ class Engine:
             out = torch.full((B, max_new_tokens), pad_token_id, device=dev, dtype=torch.int64)
             finished.zero_()
             pad = torch.full((B,), pad_token_id, device=dev, dtype=torch.int64)
-            tok = ops.argmax_rows(logits)
+            graph_key = (int(eos_token_id), int(pad_token_id))
+            if sampler:
+                # The generated-token bitmap starts empty (HF's input_ids are empty when generate gets only
+                # inputs_embeds); seed and step live on the device, so the captured decode graph draws fresh numbers.
+                V = logits.shape[1]
+                if "seen" not in st:
+                    st["seen"] = torch.zeros((B, (V + 31) // 32), device=dev, dtype=torch.int32)
+                    st["seed_dev"] = torch.zeros((1,), device=dev, dtype=torch.int64)
+                    st["step_dev"] = torch.zeros((1,), device=dev, dtype=torch.int32)
+                seen, seed_dev, step_dev = st["seen"], st["seed_dev"], st["step_dev"]
+                seen.zero_()
+                step_dev.zero_()
+                s64 = (int(seed or 0) & (2 ** 64 - 1))
+                seed_dev.fill_(s64 - 2 ** 64 if s64 >= 2 ** 63 else s64)
+                cfg = dict(do_sample=do_sample, repetition_penalty=float(repetition_penalty),
+                           temperature=float(temperature), top_k=int(top_k), top_p=float(top_p))
+                graph_key += tuple(cfg.values())
+
+                def pick(lg):
+                    t = ops.sample_rows(lg, seen, seed_dev=seed_dev, step_dev=step_dev, **cfg)
+                    step_dev.add_(1)
+                    return t
+            else:
+                pick = ops.argmax_rows
+            tok = pick(logits)
             out[:, 0] = tok
             finished |= tok == eos_token_id
             n = 1
@@ -758,13 +797,15 @@ class Engine:
                 def decode_step():
                     x1 = ops.embed_gather(table, tok_in)  # ids beyond the table (pad of finished rows) are clamped
                     x1 = self._llama_layers(x1, B, 1, None, 1, cache, t_max, pos_dev)
-                    nxt = ops.argmax_rows(self._lm_head(x1))
+                    nxt = pick(self._lm_head(x1))
                     nxt = torch.where(finished, pad_t, nxt)  # HF: finished rows emit pad
                     finished.logical_or_(nxt == eos_t)
                     tok_in.copy_(nxt)
                     pos_dev.add_(1)
 
-                graph = st["graph"] if st.get("graph_key") == (eos_t, int(pad_token_id)) else None
+                # one captured decode step per (eos, pad[, sampling configuration]): alternating greedy and sampled
+                # calls replay their own graphs
+                graph = st["graphs"].get(graph_key, (None,))[0]
                 if graph is None:
                     decode_step()  # eager first step: fills weight caches / function attributes, and is a real step
                     out[:, 1] = tok_in
@@ -773,7 +814,6 @@ class Engine:
                     if n % 8 == 2 and bool(finished.all()):  # host check every 8 steps (finished rows only emit pad)
                         break
                     if graph is None:
-                        st["pad"] = pad_t  # keep the captured pad tensor alive with the graph
                         graph = torch.cuda.CUDAGraph()
                         prof, ops.PROFILE = ops.PROFILE, None
                         try:
@@ -781,7 +821,7 @@ class Engine:
                                 decode_step()
                         finally:
                             ops.PROFILE = prof
-                        st["graph"], st["graph_key"] = graph, (eos_t, int(pad_token_id))
+                        st["graphs"][graph_key] = (graph, pad_t)  # the captured pad tensor lives with its graph
                     graph.replay()
                     out[:, n] = tok_in
                     n += 1

@@ -18,10 +18,48 @@ from typing import Optional
 import torch
 from torch import nn
 from transformers import CLIPConfig, CLIPModel, LlamaConfig, WhisperConfig, WhisperModel
-from transformers import PretrainedConfig, PreTrainedModel
+from transformers import GenerationConfig, PretrainedConfig, PreTrainedModel
 from transformers.modeling_outputs import CausalLMOutputWithPast
 
 from .engine import Engine
+
+# GenerationConfig fields that would add a logits processor, a stopping criterion or another search to HF generate,
+# with the test that they are set.  The generate branch implements greedy search and multinomial sampling with
+# repetition penalty / temperature / top-k / top-p only, so these are refused rather than ignored.
+_UNSUPPORTED_GENERATION = {
+    "num_beams": lambda v: v > 1, "num_beam_groups": lambda v: v > 1, "diversity_penalty": lambda v: v != 0.0,
+    "num_return_sequences": lambda v: v > 1, "penalty_alpha": lambda v: v is not None,
+    "dola_layers": lambda v: v is not None, "guidance_scale": lambda v: v != 1, "constraints": lambda v: bool(v),
+    "force_words_ids": lambda v: bool(v), "min_length": lambda v: v > 0, "min_new_tokens": lambda v: v > 0,
+    "no_repeat_ngram_size": lambda v: v > 0, "encoder_no_repeat_ngram_size": lambda v: v > 0,
+    "encoder_repetition_penalty": lambda v: v != 1.0, "typical_p": lambda v: v < 1.0, "min_p": lambda v: True,
+    "top_h": lambda v: True, "epsilon_cutoff": lambda v: v > 0.0, "eta_cutoff": lambda v: v > 0.0,
+    "bad_words_ids": lambda v: True, "suppress_tokens": lambda v: True, "begin_suppress_tokens": lambda v: True,
+    "sequence_bias": lambda v: True, "forced_bos_token_id": lambda v: True, "forced_eos_token_id": lambda v: True,
+    "remove_invalid_values": lambda v: bool(v), "exponential_decay_length_penalty": lambda v: True,
+    "renormalize_logits": lambda v: bool(v), "watermarking_config": lambda v: True, "stop_strings": lambda v: True,
+    "max_time": lambda v: True, "token_healing": lambda v: bool(v), "prompt_lookup_num_tokens": lambda v: True,
+}
+
+
+def generation_settings(generation_config) -> dict:
+    """Decoding keyword arguments of Engine.generate from an HF GenerationConfig, resolved as HF generate resolves them:
+    an unset (None) field takes the installed transformers' default (GenerationConfig._get_default_generation_params()).
+    A field that would change the search or add another logits processor raises NotImplementedError naming it."""
+    defaults = GenerationConfig._get_default_generation_params()
+
+    def get(name):
+        v = getattr(generation_config, name, None)
+        return defaults.get(name) if v is None else v
+
+    for name, is_set in _UNSUPPORTED_GENERATION.items():
+        v = get(name)
+        if v is not None and is_set(v):
+            raise NotImplementedError(f"macaw_b200: generation_config.{name} = {v!r} is not supported by the generate "
+                                      f"branch (greedy search or sampling with repetition_penalty / temperature / "
+                                      f"top_k / top_p only)")
+    return dict(do_sample=bool(get("do_sample")), temperature=float(get("temperature")), top_k=int(get("top_k") or 0),
+                top_p=float(get("top_p")), repetition_penalty=float(get("repetition_penalty")))
 
 
 # ---------------------------------------------------------------------------------------------------- config
@@ -195,6 +233,9 @@ class LlamaForCausalLM(_LlamaPreTrained):
         self.lm_head = nn.Linear(config.hidden_size, config.vocab_size, bias=False)
         self._engine_ref = _EngineRef()
         self.post_init()
+        # read by MM_LLMs' generate branch as HF generate reads it (this class is not a GenerationMixin, so transformers
+        # leaves the attribute None); assignable, e.g. from a checkpoint's generation_config.json
+        self.generation_config = GenerationConfig.from_model_config(config)
 
     def get_input_embeddings(self):
         return self.model.embed_tokens
@@ -321,12 +362,14 @@ class MM_LLMs(PreTrainedModel):
     def forward(self, inputs=None):
         """inputs: dict with images (B,3,H,W) | None, audios (B,80,3000) | None, videos (B,F,3,H,W) | None,
         input_ids (B,L), optional attention_mask (B,L), labels (B,L) | None, {image,audio,video}_{starts,ends} (B,),
-        optional `inference: True` (greedy generation, returns token ids; `max_new_tokens` defaults to the reference's 128)
-        (reference modeling.py:941-963, llm_trainer.py:366-381)."""
+        optional `inference: True` (generation, returns token ids; `max_new_tokens` defaults to the reference's 128;
+        greedy or sampled as `self.llm.generation_config` says) (reference modeling.py:941-963, llm_trainer.py:366-381)."""
         if inputs.get("inference") is True:
-            # generate branch (reference modeling.py:954-960): greedy decode, returns the new token ids (B, <= 128)
+            # generate branch (reference modeling.py:954-960): greedy or sampled decode, returns the new token ids
+            # (B, <= 128); every other decoding parameter comes from llm.generation_config, as in HF generate
             return self._engine.generate(inputs, max_new_tokens=int(inputs.get("max_new_tokens", 128)),
-                                         eos_token_id=2, pad_token_id=32006)
+                                         eos_token_id=2, pad_token_id=32006,
+                                         **generation_settings(self.llm.generation_config))
         if self.training and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             return self._forward_train(inputs)
         loss, logits, _, _, _ = self._engine.forward(inputs)

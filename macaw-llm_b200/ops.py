@@ -556,6 +556,27 @@ def argmax_rows(logits: torch.Tensor) -> torch.Tensor:
     return out
 
 
+def sample_rows(logits: torch.Tensor, seen: torch.Tensor, *, do_sample: bool, repetition_penalty: float = 1.0,
+                temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0, seed_dev: Optional[torch.Tensor] = None,
+                step_dev: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Next token per row of 16-bit logits (rows, V) under HF's repetition penalty / temperature / top-k / top-p chain
+    (mm_sample_rows) -> int64 (rows,).  seen: int32 (rows, ceil(V/32)) bitmap of the tokens generated so far, updated
+    in place with the emitted token.  seed_dev (int64 (1,)) and step_dev (int32 (1,)) are read on the device, so a
+    captured CUDA graph draws fresh numbers when they change; greedy (do_sample=False) does not read them."""
+    _cuda(logits, ACT(), "logits"); _cuda(seen, torch.int32, "seen")
+    assert logits.dim() == 2 and logits.stride(1) == 1
+    rows, V = logits.shape
+    assert seen.is_contiguous() and tuple(seen.shape) == (rows, (V + 31) // 32)
+    if do_sample:
+        _cuda(seed_dev, torch.int64, "seed_dev"); _cuda(step_dev, torch.int32, "step_dev")
+    out = torch.empty((rows,), device=logits.device, dtype=torch.int64)
+    _check(_lib.load().mm_sample_rows(logits.data_ptr(), logits.stride(0), rows, V, seen.data_ptr(),
+                                      float(repetition_penalty), float(temperature), int(top_k), float(top_p),
+                                      int(bool(do_sample)), _ptr(seed_dev), _ptr(step_dev), out.data_ptr(), _stream()),
+           "mm_sample_rows")
+    return out
+
+
 # ---------------------------------------------------------------------------------------------------- loss
 def ce_loss(logits: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
     """Shifted CE (mean over labels != -100) of bf16 logits (B, T, V) against int64 labels (B, T); returns fp32 scalar."""
