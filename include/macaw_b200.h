@@ -173,6 +173,7 @@ int32_t mm_splitk_reduce(const float* partial, int32_t splits, int32_t M, int32_
  * video_long_self_attention modeling.py:1078 (two synthetic keys are materialised by the caller).
  * q/k/v/out: bf16 with element strides (batch, token, head); head_dim contiguous, head_dim in {64, 96, 128}.
  * key_mask: int32 [B][Tk] (1 = attend, 0 = masked) or NULL.  causal: key j visible to query i iff j <= i + (Tk - Tq).
+ * scale > 0.
  */
 typedef struct mm_attn_args {
   const void *q, *k, *v;
@@ -185,9 +186,8 @@ typedef struct mm_attn_args {
   const int32_t* key_mask;
   int32_t causal;
   float scale;
-  int32_t impl; /* 0 = wgmma kernel (head_dim 64 / 96 / 128); 1 = force the mma.sync kernel (tests only) */
   const int32_t* tk_dev; /* NULL, or device int holding the number of valid keys (<= Tk, which then is the capacity of
-                            k / v): lets one captured launch serve a growing KV cache (wgmma kernel only) */
+                            k / v): lets one captured launch serve a growing KV cache */
 } mm_attn_args;
 int32_t mm_attn_fwd(const mm_attn_args* args, void* stream);
 
@@ -265,19 +265,6 @@ typedef struct mm_align_args {
 int32_t mm_align_fwd(const mm_align_args* args, void* stream);
 int64_t mm_align_workspace_bytes(int32_t R, int32_t V);
 
-/* ------------------------------------------------------------------------------------------------ alignment softmax
- * Row softmax of the absorbed-form alignment scores (torch F.multi_head_attention_forward: softmax over S = V + 2 keys,
- * functional.py:6531-6537, 6585-6602, 6630-6650).  scores fp32 [R][V] hold q~ . table[v]; the kernel adds row_bias[r]
- * (q_h . b_k[h]; read at row_bias[r * stat_stride], same stride for extra_score) to every real key, includes the bias_k key (score extra_score[r]) and the zero key (score 0) in the
- * normaliser, and writes P bf16 [R][V] (row stride ldp), p_sum_real[r] = sum_v P[r,v] and p_extra[r] = P of the bias_k key. */
-int32_t mm_align_softmax(const float* scores, int64_t lds, const float* row_bias, const float* extra_score,
-                         int64_t stat_stride, void* P, int64_t ldp, float* p_sum_real, float* p_extra, int32_t R,
-                         int32_t V, void* stream);
-/* Value-side bias terms of the absorbed form (functional.py:6531-6537: bias_v is appended un-projected; b_v rides on
- * every real key):  ctx[n, h*hd + d] += p_sum_real[h*Nq + n] * b_v[h*hd + d] + p_extra[h*Nq + n] * bias_v[h*hd + d]. */
-int32_t mm_align_ctx_fixup(void* ctx, int64_t ldc, const float* p_sum_real, const float* p_extra, const void* b_v,
-                           const void* bias_v, int32_t Nq, int32_t E, int32_t head_dim, void* stream);
-
 /* ------------------------------------------------------------------------------------------------ decode (generate branch)
  * Greedy decoding behind inputs['inference'] = True (reference modeling.py:954-960 -> HF generate, vendored KV-cache
  * logic modeling.py:190-195).  mm_kv_append copies the K and V thirds of a fused [q|k|v] activation (rows (b, t),
@@ -300,17 +287,10 @@ int32_t mm_argmax_rows(const void* logits, int64_t ld, int32_t rows, int32_t V, 
 int32_t mm_sample_rows(const void* logits, int64_t ld, int32_t rows, int32_t V, uint32_t* seen, float repetition_penalty,
                        float temperature, int32_t top_k, float top_p, int32_t do_sample, const uint64_t* seed_dev,
                        const int32_t* step_dev, int64_t* out, void* stream);
-/* Thin-row companions of the swapped-operand decode GEMMs (mm_gemm_args.c_trans), whose epilogue cannot pair columns:
- * mm_rope_rows: in-place rotate-half RoPE (head_dim 128, apply_rotary_pos_emb modeling.py:83-91) on the first rot_cols
- * columns; position of row r = (*pos_dev if given) + r % rope_T.  mm_swiglu_rows: out[r, j] = silu(gate_j) * up_j from
- * the [32 gate | 32 up]-interleaved product (LlamaMLP modeling.py:139-140). */
-/* Split-K tail of a thin (decode) GEMM: part fp32 [splits][N][ldp] holds W_s x_s^T per K slice (mm_gemm_fwd with the
- * operands swapped, batch = splits, fp32 out); out[m][n] = row_scale[m] * sum_s part[s][n][m] (+ residual[m][n]), bf16.
- * Splitting K lets the 32-tile o_proj / down_proj grids of a decode step cover all 132 SMs (weight streaming). */
-int32_t mm_thin_reduce(const float* part, int32_t splits, int32_t N, int32_t M, int32_t ldp, const float* row_scale,
-                       const void* residual, int64_t ldr, void* out, int64_t ldo, void* stream);
-/* Fused tail of a split-K thin GEMM — one launch instead of mm_thin_reduce + mm_rope_rows + mm_kv_append /
- * mm_swiglu_rows / mm_rms_rstd (a decode step is launch-bound: 14 -> 9 kernels per LLaMA layer):
+/* Fused tail of a split-K thin (decode) GEMM: part fp32 [splits][N][ldp] holds W_s x_s^T per K slice (mm_gemm_fwd with
+ * the operands swapped, batch = splits, fp32 out).  Splitting K lets the 32-tile o_proj / down_proj grids of a decode step
+ * cover all 132 SMs (weight streaming); one launch per GEMM finishes the sum and the ops around it (a decode step is
+ * launch-bound):
  *   MM_THIN_RES     out = rs * sum_s part + residual; sumsq_out (optional, [M][N/32]) = per-(row, 32-column) sums of squares
  *                   of the stored values, the next RMSNorm's statistic (LlamaRMSNorm modeling.py:311-319)
  *   MM_THIN_SWIGLU  out[m][32q+i] = silu(gate) * up from the [32 gate | 32 up]-interleaved product (modeling.py:139-140)
@@ -339,9 +319,11 @@ typedef struct mm_thin_args {
   const int32_t* t0_dev;
 } mm_thin_args;
 int32_t mm_thin_fused(const mm_thin_args* args, void* stream);
+/* In-place rotate-half RoPE (head_dim 128, apply_rotary_pos_emb modeling.py:83-91) on the first rot_cols columns of each
+ * row; position of row r = (*pos_dev if given) + r % rope_T.  The training step's RoPE backward calls it with the sin
+ * table negated (the rotation is orthogonal: its transpose is the rotation by -theta). */
 int32_t mm_rope_rows(void* x, int64_t ld, int32_t rows, int32_t rot_cols, const float* cos_t, const float* sin_t,
                      int32_t rope_T, const int32_t* pos_dev, void* stream);
-int32_t mm_swiglu_rows(const void* gu, int64_t ld, int32_t rows, int32_t I, void* out, int64_t ldo, void* stream);
 
 /* ------------------------------------------------------------------------------------------------ loss
  * Shifted cross entropy of LlamaForCausalLM.forward modeling.py:600-610: logits bf16 (B, T, V), labels int64 (B, T);

@@ -61,7 +61,7 @@ class AttnArgs(C.Structure):
         ("k_bs", c_i64), ("k_ts", c_i64), ("k_hs", c_i64),
         ("v_bs", c_i64), ("v_ts", c_i64), ("v_hs", c_i64),
         ("o_bs", c_i64), ("o_ts", c_i64), ("o_hs", c_i64),
-        ("key_mask", c_vp), ("causal", c_i32), ("scale", c_f32), ("impl", c_i32), ("tk_dev", c_vp),
+        ("key_mask", c_vp), ("causal", c_i32), ("scale", c_f32), ("tk_dev", c_vp),
     ]
 
 
@@ -121,18 +121,14 @@ SIGNATURES = {
     "mm_copy_rows": (c_i32, [c_vp, c_i64, c_vp, c_i64, c_i32, c_i32, c_vp]),
     "mm_align_fwd": (c_i32, [C.POINTER(AlignArgs), c_vp]),
     "mm_align_workspace_bytes": (c_i64, [c_i32, c_i32]),
-    "mm_align_softmax": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp, c_vp, c_i32, c_i32, c_vp]),
-    "mm_align_ctx_fixup": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_i32, c_vp]),
     "mm_kv_append": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp]),
     "mm_gemm_streamk_workspace_bytes": (c_i64, []),
     "mm_gemm_streamk_mode": (c_i32, [c_i32]),
     "mm_gemm_overlap_mode": (c_i32, [c_i32]),
     "mm_thin_fused": (c_i32, [C.POINTER(ThinArgs), c_vp]),
-    "mm_thin_reduce": (c_i32, [c_vp, c_i32, c_i32, c_i32, c_i32, c_vp, c_vp, c_i64, c_vp, c_i64, c_vp]),
     "mm_argmax_rows": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_vp]),
     "mm_sample_rows": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_f32, c_f32, c_i32, c_f32, c_i32, c_vp, c_vp, c_vp, c_vp]),
     "mm_rope_rows": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp]),
-    "mm_swiglu_rows": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_i64, c_vp]),
     "mm_rmsnorm_bwd": (c_i32, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_i32, c_i32, c_vp]),
     "mm_rmsnorm_bwd_parts": (c_i32, [c_i32]),
     "mm_swiglu_fwd": (c_i32, [c_vp, c_vp, c_vp, c_i64, c_vp]),
@@ -176,7 +172,7 @@ SIGNATURES = {
 NULLABLE_BEFORE_STREAM = {"mm_adamw": 1, "mm_adamw_host": 1}
 
 _lib = None
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 
 class _NullableBeforeStream:

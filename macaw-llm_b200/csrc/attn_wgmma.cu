@@ -14,7 +14,7 @@
 // Reference call sites replaced: see include/macaw_b200.h (mm_attn_fwd).  head_dim 96 (video-long self-attention,
 // reference modeling.py:1078) runs on the HD = 128 instantiation: the Q / K / V tensor maps carry the real head dim, so
 // the TMA boxes of the second 64-column block are zero-filled past column 96; S = Q K^T issues 6 of 8 k-steps and the
-// zero columns of O are not stored.  The mma.sync kernel in attn.cu is kept as a second implementation for tests.
+// zero columns of O are not stored.
 #include "common.cuh"
 #include "ptx.cuh"
 #include "../../include/macaw_b200.h"
@@ -327,10 +327,23 @@ static int launch_fa(const mm_attn_args* a, cudaStream_t st) {
   return check_launch("mm_attn_fwd(wgmma)");
 }
 
-// called from mm_attn_fwd (attn.cu) for head_dim 64 / 96 / 128 when scale > 0 (96 rides the 128 instantiation)
-int attn_wgmma_dispatch(const mm_attn_args* a, cudaStream_t st) {
+}  // namespace mm
+using namespace mm;
+
+extern "C" int32_t mm_attn_fwd(const mm_attn_args* a, void* stream) {
+  MM_REQUIRE(a && a->q && a->k && a->v && a->out, "mm_attn_fwd: null argument");
+  MM_REQUIRE(a->B > 0 && a->H > 0 && a->Tq > 0 && a->Tk > 0, "mm_attn_fwd: bad shape");
+  MM_REQUIRE(a->head_dim == 64 || a->head_dim == 96 || a->head_dim == 128, "mm_attn_fwd: head_dim %d unsupported",
+             a->head_dim);
+  MM_REQUIRE(a->scale > 0.f, "mm_attn_fwd: scale must be positive");
+  const int64_t strides[] = {a->q_bs, a->q_ts, a->q_hs, a->k_bs, a->k_ts, a->k_hs,
+                             a->v_bs, a->v_ts, a->v_hs, a->o_bs, a->o_ts, a->o_hs};
+  for (int64_t s : strides) MM_REQUIRE(s % 8 == 0, "mm_attn_fwd: strides must be multiples of 8 elements");
+  MM_REQUIRE(((uintptr_t)a->q % 16 == 0) && ((uintptr_t)a->k % 16 == 0) && ((uintptr_t)a->v % 16 == 0) &&
+                 ((uintptr_t)a->out % 16 == 0),
+             "mm_attn_fwd: pointers must be 16-byte aligned");
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  // head_dim 96 rides the 128 instantiation
   if (act_f16()) return a->head_dim == 64 ? launch_fa<64, true>(a, st) : launch_fa<128, true>(a, st);
   return a->head_dim == 64 ? launch_fa<64, false>(a, st) : launch_fa<128, false>(a, st);
 }
-
-}  // namespace mm

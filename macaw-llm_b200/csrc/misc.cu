@@ -321,102 +321,6 @@ __global__ void cast_bf16_f16_kernel(const bf16* __restrict__ x, long long ldx, 
   }
 }
 
-// ------------------------------------------------------------------------------------------------ alignment softmax
-// one CTA per score row.  See mm_align_softmax in the header for the exact semantics.
-__global__ void __launch_bounds__(512) align_softmax_kernel(const float* __restrict__ scores, long long lds,
-                                                            const float* __restrict__ row_bias,
-                                                            const float* __restrict__ extra_score, long long sstride,
-                                                            bf16* __restrict__ P, long long ldp,
-                                                            float* __restrict__ p_sum_real, float* __restrict__ p_extra,
-                                                            int V) {
-  __shared__ float sh[32];
-  const long long r = blockIdx.x;
-  const float* s = scores + r * lds;
-  const float rb = row_bias ? row_bias[r * sstride] : 0.f;
-  const float ex = extra_score[r * sstride];
-  const bool vec = (lds % 4 == 0) && ((reinterpret_cast<uintptr_t>(scores) & 15) == 0);
-  // pass 1: running max / sum of exp (online, per thread), in the log2 domain
-  constexpr float L2E = 1.4426950408889634f;
-  float m = -INFINITY, l = 0.f;
-  if (vec) {
-    const int n4 = V >> 2;
-    for (int c = threadIdx.x; c < n4; c += blockDim.x) {
-      const float4 v4 = *reinterpret_cast<const float4*>(s + 4 * c);
-      const float mx = fmaxf(fmaxf(v4.x, v4.y), fmaxf(v4.z, v4.w));
-      if (mx > m) {
-        l *= exp2f((m - mx) * L2E);
-        m = mx;
-      }
-      l += exp2f((v4.x - m) * L2E) + exp2f((v4.y - m) * L2E) + exp2f((v4.z - m) * L2E) + exp2f((v4.w - m) * L2E);
-    }
-    for (int c = (n4 << 2) + threadIdx.x; c < V; c += blockDim.x) {
-      const float v = s[c];
-      if (v > m) {
-        l *= exp2f((m - v) * L2E);
-        m = v;
-      }
-      l += exp2f((v - m) * L2E);
-    }
-  } else {
-    for (int c = threadIdx.x; c < V; c += blockDim.x) {
-      const float v = s[c];
-      if (v > m) {
-        l *= exp2f((m - v) * L2E);
-        m = v;
-      }
-      l += exp2f((v - m) * L2E);
-    }
-  }
-  const float m_real = block_max(m, sh);  // max over real keys (before row bias)
-  l = (m == -INFINITY) ? 0.f : l * exp2f((m - m_real) * L2E);
-  const float l_real = block_sum(l, sh);  // sum_v exp(s_v - m_real)
-  // fold in the two synthetic keys: bias_k key (score ex) and the zero key (score 0)
-  const float m_all = fmaxf(fmaxf(m_real + rb, ex), 0.f);
-  const float e_real = exp2f((m_real + rb - m_all) * L2E);  // rescale of the real-key sum
-  const float e_ex = exp2f((ex - m_all) * L2E);
-  const float e_zero = exp2f((0.f - m_all) * L2E);
-  const float denom = l_real * e_real + e_ex + e_zero;
-  const float inv = 1.0f / denom;
-  if (threadIdx.x == 0) {
-    p_sum_real[r] = l_real * e_real * inv;
-    p_extra[r] = e_ex * inv;
-  }
-  // pass 2: P = exp(s + rb - m_all) / denom
-  bf16* pr = P + r * ldp;
-  const float off = rb - m_all;
-  if (vec && (ldp % 4 == 0)) {
-    const int n4 = V >> 2;
-    for (int c = threadIdx.x; c < n4; c += blockDim.x) {
-      const float4 v4 = *reinterpret_cast<const float4*>(s + 4 * c);
-      uint2 u;
-      u.x = pack_bf16x2(exp2f((v4.x + off) * L2E) * inv, exp2f((v4.y + off) * L2E) * inv);
-      u.y = pack_bf16x2(exp2f((v4.z + off) * L2E) * inv, exp2f((v4.w + off) * L2E) * inv);
-      *reinterpret_cast<uint2*>(pr + 4 * c) = u;
-    }
-    for (int c = (n4 << 2) + threadIdx.x; c < V; c += blockDim.x)
-      pr[c] = __float2bfloat16(exp2f((s[c] + off) * L2E) * inv);
-  } else {
-    for (int c = threadIdx.x; c < V; c += blockDim.x) pr[c] = __float2bfloat16(exp2f((s[c] + off) * L2E) * inv);
-  }
-  // zero the alignment padding of the row so that the K tail of the P.table GEMM reads zeros
-  for (int c = V + threadIdx.x; c < ldp; c += blockDim.x) pr[c] = __float2bfloat16(0.f);
-}
-
-// ctx[n, h*hd + d] += psum[h*Nq + n] * b_v[h*hd + d] + pextra[h*Nq + n] * bias_v[h*hd + d]
-__global__ void align_ctx_fixup_kernel(bf16* __restrict__ ctx, long long ldc, const float* __restrict__ psum,
-                                       const float* __restrict__ pextra, const bf16* __restrict__ b_v,
-                                       const bf16* __restrict__ bias_v, int Nq, int E, int hd) {
-  const long long total = static_cast<long long>(Nq) * E;
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int n = static_cast<int>(i / E), e = static_cast<int>(i % E), h = e / hd;
-    const long long r = static_cast<long long>(h) * Nq + n;
-    const float v = __bfloat162float(ctx[n * ldc + e]) + psum[r] * __bfloat162float(b_v[e]) +
-                    pextra[r] * __bfloat162float(bias_v[e]);
-    ctx[n * ldc + e] = __float2bfloat16(v);
-  }
-}
-
 // ------------------------------------------------------------------------------------------------ decode helpers
 // K / V rows of a fused QKV activation -> per-layer cache (B, Tmax, 2, E) at positions t0 .. t0 + T_new - 1
 __global__ void __launch_bounds__(128) kv_append_kernel(const bf16* __restrict__ qkv, long long ld_qkv, int T_new, int E,
@@ -431,8 +335,9 @@ __global__ void __launch_bounds__(128) kv_append_kernel(const bf16* __restrict__
   for (int c = threadIdx.x; c < (2 * E) >> 3; c += blockDim.x) d4[c] = s4[c];
 }
 
-// rotate-half RoPE (head_dim 128) in place on the first `rot_cols` columns of thin rows (decode step): position of row r
-// = pos_base (+ *pos_dev) + r % rope_T.  Same arithmetic as the GEMM's RoPE epilogue (fp32, tables (T, 64)).
+// rotate-half RoPE (head_dim 128) in place on the first `rot_cols` columns of each row: position of row r
+// = (*pos_dev if given) + r % rope_T.  Same arithmetic as the GEMM's RoPE epilogue (fp32, tables (T, 64)); with negated sin
+// tables it applies the transposed rotation of the training step's RoPE backward.
 template <bool F16>
 __global__ void rope_rows_kernel(bf16* __restrict__ x, long long ld, int rows, int rot_cols, const float* __restrict__ cs,
                                  const float* __restrict__ sn, int rope_T, const int* __restrict__ pos_dev) {
@@ -452,38 +357,6 @@ __global__ void rope_rows_kernel(bf16* __restrict__ x, long long ld, int rows, i
   }
 }
 
-// out[r, 32 q + i] = silu(gu[r, 64 q + i]) * gu[r, 64 q + 32 + i]: the [32 gate | 32 up] interleave of the fused weight
-template <bool F16>
-__global__ void swiglu_rows_kernel(const bf16* __restrict__ gu, long long ld, int rows, int I, bf16* __restrict__ out,
-                                   long long ldo) {
-  const long long total = static_cast<long long>(rows) * I;
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int r = static_cast<int>(i / I), c = static_cast<int>(i % I);
-    const bf16* g = gu + r * ld + (c / 32) * 64 + (c % 32);
-    const float a = ldv<F16>(g[0]), b = ldv<F16>(g[32]);
-    out[r * ldo + c] = stv<F16>(a / (1.0f + __expf(-a)) * b);
-  }
-}
-
-// Tail of the split-K thin GEMMs of a decode step: part[s][n][m] fp32 (the swapped-operand product W_s x_s^T per K slice)
-// -> out[m][n] = act_scale[m] * sum_s part[s][n][m] (+ residual[m][n]), bf16.
-template <bool F16>
-__global__ void thin_reduce_kernel(const float* __restrict__ part, int S, int N, int M, int ldp,
-                                   const float* __restrict__ row_scale, const bf16* __restrict__ residual, long long ldr,
-                                   bf16* __restrict__ out, long long ldo) {
-  const long long total = static_cast<long long>(N) * M;
-  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int n = static_cast<int>(i / M), m = static_cast<int>(i % M);
-    float acc = 0.f;
-    for (int s = 0; s < S; ++s) acc += part[(static_cast<long long>(s) * N + n) * ldp + m];
-    if (row_scale != nullptr) acc *= row_scale[m];
-    if (residual != nullptr) acc += ldv<F16>(residual[static_cast<long long>(m) * ldr + n]);
-    out[static_cast<long long>(m) * ldo + n] = stv<F16>(acc);
-  }
-}
-
 // Fused tail of a split-K thin GEMM (decode step): one warp per unit of 32 (or 2 x 32) output features, all M rows.
 //   MM_THIN_RES    out[m][n] = rs_m * sum_s part[s][n][m] + residual[m][n];  optionally the per-(row, 32-column) sums of
 //                  squares of the STORED values (the next RMSNorm's statistic — replaces a pass over the stream)
@@ -492,7 +365,7 @@ __global__ void thin_reduce_kernel(const float* __restrict__ part, int S, int N,
 //                  prefill GEMM's RoPE epilogue does —, q -> out[m][n], k / v -> straight into the layer's KV cache slot
 //                  (B, Tmax, 2, E) at position t0 (row m = sample m: one new token per sample)
 // rs_m = row_scale[m], or rsqrt(sum_j rs_sumsq[m][j] / rs_K + rs_eps) from the statistics a MM_THIN_RES pass left (fixed
-// summation order: deterministic), or 1.  Replaces thin_reduce + rope_rows + kv_append / swiglu_rows / rms_rstd launches.
+// summation order: deterministic), or 1.
 struct ThinFusedParams {
   const float* part;
   int S, N, M, ldp;
@@ -1081,28 +954,6 @@ extern "C" int32_t mm_cast_bf16_f16(const void* x, int64_t ldx, void* y, int64_t
   return check_launch("mm_cast_bf16_f16");
 }
 
-extern "C" int32_t mm_align_softmax(const float* scores, int64_t lds, const float* row_bias, const float* extra_score,
-                                    int64_t stat_stride, void* P, int64_t ldp, float* p_sum_real, float* p_extra,
-                                    int32_t R, int32_t V, void* stream) {
-  MM_REQUIRE(scores && extra_score && P && p_sum_real && p_extra && R > 0 && V > 0 && lds >= V && ldp >= V,
-             "mm_align_softmax: bad arguments");
-  align_softmax_kernel<<<R, 512, 0, ST(stream)>>>(scores, lds, row_bias, extra_score, stat_stride, (bf16*)P, ldp,
-                                                  p_sum_real, p_extra, V);
-  return check_launch("mm_align_softmax");
-}
-
-extern "C" int32_t mm_align_ctx_fixup(void* ctx, int64_t ldc, const float* p_sum_real, const float* p_extra,
-                                      const void* b_v, const void* bias_v, int32_t Nq, int32_t E, int32_t head_dim,
-                                      void* stream) {
-  MM_REQUIRE(ctx && p_sum_real && p_extra && b_v && bias_v && Nq > 0 && E > 0 && head_dim > 0 && E % head_dim == 0,
-             "mm_align_ctx_fixup: bad arguments");
-  const long long total = static_cast<long long>(Nq) * E;
-  align_ctx_fixup_kernel<<<grid_for(total, 256), 256, 0, ST(stream)>>>((bf16*)ctx, ldc, p_sum_real, p_extra,
-                                                                       (const bf16*)b_v, (const bf16*)bias_v, Nq, E,
-                                                                       head_dim);
-  return check_launch("mm_align_ctx_fixup");
-}
-
 extern "C" int32_t mm_kv_append(const void* qkv, int64_t ld_qkv, int32_t B, int32_t T_new, int32_t E, void* cache,
                                 int32_t Tmax, int32_t t0, const int32_t* t0_dev, void* stream) {
   MM_REQUIRE(qkv && cache && B > 0 && T_new > 0 && E > 0 && E % 8 == 0 && ld_qkv % 8 == 0 && t0 >= 0 &&
@@ -1119,25 +970,6 @@ extern "C" int32_t mm_rope_rows(void* x, int64_t ld, int32_t rows, int32_t rot_c
   auto kern = act_f16() ? rope_rows_kernel<true> : rope_rows_kernel<false>;
   kern<<<grid_for(total, 256), 256, 0, ST(stream)>>>((bf16*)x, ld, rows, rot_cols, cos_t, sin_t, rope_T, pos_dev);
   return check_launch("mm_rope_rows");
-}
-
-extern "C" int32_t mm_swiglu_rows(const void* gu, int64_t ld, int32_t rows, int32_t I, void* out, int64_t ldo, void* stream) {
-  MM_REQUIRE(gu && out && rows > 0 && I > 0 && I % 32 == 0, "mm_swiglu_rows: bad arguments");
-  const long long total = static_cast<long long>(rows) * I;
-  auto kern = act_f16() ? swiglu_rows_kernel<true> : swiglu_rows_kernel<false>;
-  kern<<<grid_for(total, 256), 256, 0, ST(stream)>>>((const bf16*)gu, ld, rows, I, (bf16*)out, ldo);
-  return check_launch("mm_swiglu_rows");
-}
-
-extern "C" int32_t mm_thin_reduce(const float* part, int32_t splits, int32_t N, int32_t M, int32_t ldp,
-                                  const float* row_scale, const void* residual, int64_t ldr, void* out, int64_t ldo,
-                                  void* stream) {
-  MM_REQUIRE(part && out && splits > 0 && N > 0 && M > 0 && ldp >= M, "mm_thin_reduce: bad arguments");
-  const long long total = static_cast<long long>(N) * M;
-  auto kern = act_f16() ? thin_reduce_kernel<true> : thin_reduce_kernel<false>;
-  kern<<<grid_for(total, 256), 256, 0, ST(stream)>>>(part, splits, N, M, ldp, row_scale,
-                                                                  (const bf16*)residual, ldr, (bf16*)out, ldo);
-  return check_launch("mm_thin_reduce");
 }
 
 extern "C" int32_t mm_thin_fused(const mm_thin_args* a, void* stream) {

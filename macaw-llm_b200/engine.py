@@ -48,7 +48,6 @@ class Engine:
         # Stream-K tail in the LLaMA GEMMs (a partial last wave of tiles is split along K over all SMs): matters at small
         # per-GPU batch (e.g. 1088 tiles on 132 SMs -> 8.2 waves), a no-op when the tile count fills the waves.
         self.streamk = True
-        self.fused_decode_tails = True  # decode step: one tail kernel per thin GEMM (mm_thin_fused) instead of 2-3 row-wise kernels
         self._sk_ws: Dict[str, torch.Tensor] = {}
         self._graphs_on = False
         self.align_max_rows = None  # test hook: cap on query rows per alignment chunk (default: ~2 GiB of fp32 scores)
@@ -599,40 +598,29 @@ class Engine:
         else:
             rope = (cos, sin, T, 2 * E) if pos0 == 0 else (cos[pos0:], sin[pos0:], 1, 2 * E)
         assert (pos0 == 0 and not dyn) or T == 1
-        # RMSNorm statistics ride the GEMM epilogues: the GEMM that WRITES the residual stream (o_proj / down_proj) leaves
-        # per-(row, 32-column) sums of squares of the stored values, the GEMM that CONSUMES it (QKV / gate-up / lm_head)
-        # derives rsqrt(mean(x^2) + eps) from them — no separate pass over the stream after the first layer's input.
+        # Decode step (one new token per sample, at most 64 samples): each GEMM swaps its operands so the weights fill the
+        # 128-row MMA tiles, splits K, and ends in ONE tail kernel that also does the neighbouring row-wise work (RoPE +
+        # KV-cache write / SwiGLU / residual + next RMSNorm statistic): 9 launches per layer.  Everything else runs the
+        # wide GEMMs, whose epilogues apply RoPE, SwiGLU and the residual adds.
+        # Either way the RMSNorm statistics ride the GEMM epilogues: the GEMM that WRITES the residual stream (o_proj /
+        # down_proj) leaves per-(row, 32-column) sums of squares of the stored values, the GEMM that CONSUMES it (QKV /
+        # gate-up / lm_head) derives rsqrt(mean(x^2) + eps) from them — no separate pass over the stream after the first
+        # layer's input.
         M = x.shape[0]
-        fused_stats = not (T == 1 and B * T <= 64) and E % 128 == 0
-        ss_attn = torch.empty((M, E // 32), device=dev, dtype=torch.float32) if fused_stats else None
-        ss_mlp = torch.empty((M, E // 32), device=dev, dtype=torch.float32) if fused_stats else None
-        have_ss = False
+        decode = cache is not None and T == 1 and B <= 64
+        ss_attn = torch.empty((M, E // 32), device=dev, dtype=torch.float32)
+        ss_mlp = torch.empty((M, E // 32), device=dev, dtype=torch.float32)
         for i, l in enumerate(self.m.llm.model.layers):
             wqkv, wgu, wo, wd = self._llama_weights(i, l, E, I)
-            thin = T == 1 and B * T <= 64  # decode step: swap operands so the weights fill the 128-row MMA tiles
-            fused_thin = thin and cache is not None and self.fused_decode_tails and E % 128 == 0
-            if fused_thin:
-                # decode step, 9 launches per layer: each split-K thin GEMM is followed by ONE tail kernel that also does
-                # the neighbouring row-wise work (RoPE + KV-cache write / SwiGLU / residual + next RMSNorm statistic)
-                if i == 0:
-                    thin_ss = (torch.empty((M, E // 32), device=dev, dtype=torch.float32),
-                               torch.empty((M, E // 32), device=dev, dtype=torch.float32))
-                    rs_kw = dict(row_scale=ops.rms_rstd(x, eps))
-                else:
-                    rs_kw = dict(rms_from=(thin_ss[1], eps))
+            rs_kw = dict(row_scale=ops.rms_rstd(x, eps)) if i == 0 else dict(rms_from=(ss_mlp, eps))
+            if decode:
                 qkv = ops.linear_thin_fused(x, wqkv, ops.THIN_QKV, rope=(rope[0], rope[1], rope[4] if len(rope) > 4 else None),
                                             cache=cache[i], t0=pos0, t0_dev=pos_dev[0:1] if dyn else None, **rs_kw)
-            elif thin:
-                rstd = ops.rms_rstd(x, eps)
-                qkv = ops.linear_thin_splitk(x, wqkv, row_scale=rstd)
-                ops.rope_rows(qkv, 2 * E, rope[0], rope[1], rope[2], rope[4] if len(rope) > 4 else None)
-            elif have_ss:
-                qkv = ops.linear(x, wqkv, epi=ops.EPI_ROPE, rope=rope, rms_from=(ss_mlp, eps))
             else:
-                qkv = ops.linear(x, wqkv, epi=ops.EPI_ROPE, rope=rope, row_scale=ops.rms_rstd(x, eps))
+                qkv = ops.linear(x, wqkv, epi=ops.EPI_ROPE, rope=rope, **rs_kw)
+                if cache is not None:
+                    ops.kv_append(qkv, B, T, cache[i], pos0, pos_dev[0:1] if dyn else None)
             q5 = qkv.view(B, T, 3, H, hd)
-            if cache is not None and not fused_thin:
-                ops.kv_append(qkv, B, T, cache[i], pos0, pos_dev[0:1] if dyn else None)
             if dyn:
                 kv = cache[i].unflatten(-1, (H, hd))  # whole capacity; the kernel reads the valid length from pos_dev[1]
                 a = ops.attention(q5[:, :, 0], kv[:, :, 0], kv[:, :, 1], scale=scale, causal=False, key_mask=kmask,
@@ -642,25 +630,15 @@ class Engine:
             else:
                 kv = cache[i][:, : pos0 + T].unflatten(-1, (H, hd))  # (B, Tk, 2, H, hd) view of the cache
                 a = ops.attention(q5[:, :, 0], kv[:, :, 0], kv[:, :, 1], scale=scale, causal=False, key_mask=kmask)
-            if fused_thin:
-                ops.linear_thin_fused(a.view(B * T, E), wo, ops.THIN_RES, residual=x, out=x, sumsq_out=thin_ss[0])
-                g = ops.linear_thin_fused(x, wgu, ops.THIN_SWIGLU, rms_from=(thin_ss[0], eps))
-                ops.linear_thin_fused(g, wd, ops.THIN_RES, residual=x, out=x, sumsq_out=thin_ss[1])
-            elif thin:
-                ops.linear_thin_splitk(a.view(B * T, E), wo, residual=x, out=x)
-                rstd = ops.rms_rstd(x, eps)
-                g = ops.swiglu_rows(ops.linear_thin_splitk(x, wgu, row_scale=rstd), I)
-                ops.linear_thin_splitk(g, wd, residual=x, out=x)
-            elif fused_stats:
+            if decode:
+                ops.linear_thin_fused(a.view(B * T, E), wo, ops.THIN_RES, residual=x, out=x, sumsq_out=ss_attn)
+                g = ops.linear_thin_fused(x, wgu, ops.THIN_SWIGLU, rms_from=(ss_attn, eps))
+                ops.linear_thin_fused(g, wd, ops.THIN_RES, residual=x, out=x, sumsq_out=ss_mlp)
+            else:
                 ops.linear(a.view(B * T, E), wo, residual=x, out=x, sumsq_out=ss_attn)
                 g = ops.linear(x, wgu, epi=ops.EPI_SWIGLU, rms_from=(ss_attn, eps))
                 ops.linear(g, wd, residual=x, out=x, sumsq_out=ss_mlp)
-                have_ss = True
-            else:
-                ops.linear(a.view(B * T, E), wo, residual=x, out=x)
-                g = ops.linear(x, wgu, epi=ops.EPI_SWIGLU, row_scale=ops.rms_rstd(x, eps))
-                ops.linear(g, wd, residual=x, out=x)
-        self._last_ss = ss_mlp if have_ss else None  # statistics of the final residual stream (consumed by _lm_head)
+        self._last_ss = None if decode else ss_mlp  # statistics of the final residual stream (consumed by _lm_head)
         return x
 
     def _lm_head(self, x: torch.Tensor, rows: Optional[torch.Tensor] = None) -> torch.Tensor:

@@ -217,32 +217,6 @@ def linear_thin(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] =
 THIN_SPLITS = 4  # K slices of a thin (decode) GEMM: 32..172-tile grids become 128..688 units on 132 SMs
 
 
-def linear_thin_splitk(x: torch.Tensor, w: torch.Tensor, *, residual: Optional[torch.Tensor] = None,
-                       out: Optional[torch.Tensor] = None, row_scale: Optional[torch.Tensor] = None,
-                       splits: Optional[int] = None) -> torch.Tensor:
-    """`linear_thin` (no bias / activation) with the K dimension split over `splits` CTAs per weight tile: fp32 partials +
-    mm_thin_reduce.  Falls back to `linear_thin` when K does not split into 64-element multiples."""
-    _cuda(x, ACT(), "x"); _cuda(w, ACT(), "w")
-    M, K = x.shape
-    N = w.shape[0]
-    S = THIN_SPLITS if splits is None else int(splits)
-    if S <= 1 or K % (S * 64) != 0:
-        return linear_thin(x, w, residual=residual, out=out, row_scale=row_scale)
-    assert x.stride(1) == 1 and w.stride(1) == 1 and w.shape[1] == K
-    Kc = K // S
-    Mp = (M + 3) // 4 * 4
-    part = torch.empty((S, N, Mp), device=x.device, dtype=torch.float32)
-    gemm_raw(M=N, N=M, K=Kc, batch=S, A=w.data_ptr(), lda=w.stride(0), a_bs=Kc, B=x.data_ptr(), ldb=x.stride(0), b_bs=Kc,
-             Cout=part.data_ptr(), ldc=Mp, c_bs=N * Mp, c_fp32=True)
-    if out is None:
-        out = torch.empty((M, N), device=x.device, dtype=ACT())
-    assert out.shape == (M, N) and out.stride(1) == 1
-    _check(_lib.load().mm_thin_reduce(part.data_ptr(), S, N, M, Mp, _ptr(row_scale), _ptr(residual),
-                                      0 if residual is None else residual.stride(0), out.data_ptr(), out.stride(0),
-                                      _stream()), "mm_thin_reduce")
-    return out
-
-
 THIN_RES, THIN_SWIGLU, THIN_QKV = 0, 1, 2
 
 
@@ -313,7 +287,7 @@ def splitk_reduce(partial: torch.Tensor, bias: Optional[torch.Tensor], out: torc
 
 # ---------------------------------------------------------------------------------------------------- attention
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, *, scale: float, causal: bool = False,
-              key_mask: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None, impl: int = 0,
+              key_mask: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
               tk_dev: Optional[torch.Tensor] = None) -> torch.Tensor:
     """q (B, Tq, H, hd), k/v (B, Tk, H, hd) bf16 views (hd contiguous, arbitrary other strides) -> (B, Tq, H, hd)."""
     for n, t in (("q", q), ("k", k), ("v", v)):
@@ -329,7 +303,7 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, *, scale: float
     a = AttnArgs(q.data_ptr(), k.data_ptr(), v.data_ptr(), out.data_ptr(), B, H, Tq, Tk, hd,
                  q.stride(0), q.stride(1), q.stride(2), k.stride(0), k.stride(1), k.stride(2),
                  v.stride(0), v.stride(1), v.stride(2), out.stride(0), out.stride(1), out.stride(2),
-                 _ptr(key_mask), int(causal), float(scale), int(impl), _ptr(tk_dev))
+                 _ptr(key_mask), int(causal), float(scale), _ptr(tk_dev))
     _check(_lib.load().mm_attn_fwd(C.byref(a), _stream()), "mm_attn_fwd")
     return out
 
@@ -492,29 +466,6 @@ def align_fused(table: torch.Tensor, qt: torch.Tensor, stats: torch.Tensor, out:
     return out, psum, pext
 
 
-def align_softmax(scores: torch.Tensor, stats: torch.Tensor, P: torch.Tensor, V: int):
-    """scores fp32 (R, >=V); stats fp32 (R, 2) = [row_bias, extra_score]; P bf16 (R, ldp) -> (p_sum_real, p_extra)."""
-    _cuda(scores, torch.float32, "scores"); _cuda(stats, torch.float32, "stats"); _cuda(P, ACT(), "P")
-    R = scores.shape[0]
-    assert stats.shape == (R, 2) and stats.is_contiguous() and P.shape[0] == R
-    psum = torch.empty((R,), device=scores.device, dtype=torch.float32)
-    pext = torch.empty((R,), device=scores.device, dtype=torch.float32)
-    _check(_lib.load().mm_align_softmax(scores.data_ptr(), scores.stride(0), stats.data_ptr(), stats.data_ptr() + 4, 2,
-                                        P.data_ptr(), P.stride(0), psum.data_ptr(), pext.data_ptr(), R, V, _stream()),
-           "mm_align_softmax")
-    return psum, pext
-
-
-def align_ctx_fixup(ctx: torch.Tensor, psum: torch.Tensor, pext: torch.Tensor, b_v: torch.Tensor,
-                    bias_v: torch.Tensor, head_dim: int) -> torch.Tensor:
-    _cuda(ctx, ACT(), "ctx")
-    Nq, E = ctx.shape
-    _check(_lib.load().mm_align_ctx_fixup(ctx.data_ptr(), ctx.stride(0), psum.data_ptr(), pext.data_ptr(),
-                                          b_v.data_ptr(), bias_v.data_ptr(), Nq, E, head_dim, _stream()),
-           "mm_align_ctx_fixup")
-    return ctx
-
-
 # ---------------------------------------------------------------------------------------------------- decode helpers
 def kv_append(qkv: torch.Tensor, B: int, T_new: int, cache: torch.Tensor, t0: int,
               t0_dev: Optional[torch.Tensor] = None) -> None:
@@ -528,22 +479,12 @@ def kv_append(qkv: torch.Tensor, B: int, T_new: int, cache: torch.Tensor, t0: in
 
 def rope_rows(x: torch.Tensor, rot_cols: int, cos: torch.Tensor, sin: torch.Tensor, rope_T: int,
               pos_dev: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """In-place rotate-half RoPE (head_dim 128) on the first rot_cols columns of thin bf16 rows."""
+    """In-place rotate-half RoPE (head_dim 128) on the first rot_cols columns of 16-bit rows (x, cos and sin tables (T, 64))."""
     _cuda(x, ACT(), "x")
     assert x.dim() == 2 and x.stride(1) == 1
     _check(_lib.load().mm_rope_rows(x.data_ptr(), x.stride(0), x.shape[0], rot_cols, cos.data_ptr(), sin.data_ptr(), rope_T,
                                     _ptr(pos_dev), _stream()), "mm_rope_rows")
     return x
-
-
-def swiglu_rows(gu: torch.Tensor, I: int) -> torch.Tensor:
-    """(rows, 2I) [32 gate | 32 up]-interleaved product -> (rows, I) silu(gate) * up."""
-    _cuda(gu, ACT(), "gu")
-    assert gu.dim() == 2 and gu.stride(1) == 1 and gu.shape[1] == 2 * I
-    out = torch.empty((gu.shape[0], I), device=gu.device, dtype=ACT())
-    _check(_lib.load().mm_swiglu_rows(gu.data_ptr(), gu.stride(0), gu.shape[0], I, out.data_ptr(), out.stride(0),
-                                      _stream()), "mm_swiglu_rows")
-    return out
 
 
 def argmax_rows(logits: torch.Tensor) -> torch.Tensor:
@@ -580,14 +521,7 @@ def sample_rows(logits: torch.Tensor, seen: torch.Tensor, *, do_sample: bool, re
 # ---------------------------------------------------------------------------------------------------- loss
 def ce_loss(logits: torch.Tensor, labels: torch.Tensor) -> torch.Tensor:
     """Shifted CE (mean over labels != -100) of bf16 logits (B, T, V) against int64 labels (B, T); returns fp32 scalar."""
-    _cuda(logits, ACT(), "logits"); _cuda(labels, torch.int64, "labels")
-    assert logits.is_contiguous() and labels.is_contiguous()
-    B, T, V = logits.shape
-    acc = torch.zeros((2,), device=logits.device, dtype=torch.float32)
-    cnt = acc[1:].view(torch.int32)
-    _check(_lib.load().mm_ce_loss(logits.data_ptr(), labels.data_ptr(), B, T, V, acc.data_ptr(), cnt.data_ptr(),
-                                  _stream()), "mm_ce_loss")
-    return acc[0] / cnt[0].to(torch.float32)
+    return ce_loss_with_count(logits, labels)[0]
 
 
 # ---------------------------------------------------------------------------------------------------- training step

@@ -85,6 +85,26 @@ def test_forward_vs_golden_and_oracle(tiny, name):
         assert abs(float(out.loss) - float(o["loss"])) < 2e-2 * abs(float(o["loss"]))
 
 
+def test_one_token_forward_vs_oracle(tiny):
+    """A text-only forward of L = 1 (T == 1, B <= 64, no KV cache) runs the same wide GEMMs as any other forward; only a
+    decode step with a cache takes the thin tails."""
+    from oracle import macaw_oracle as O
+
+    model, spec, hp, weights = tiny
+    inp = H.gen.make_inputs(spec, 4, 1, seed=105, modalities=(), with_labels=False)
+    inp["input_ids"] = torch.tensor([[1], [7], [300], [55]])
+    out = model({k: (v.cuda() if isinstance(v, torch.Tensor) else v) for k, v in inp.items()})
+    torch.cuda.synchronize()
+    assert tuple(out.logits.shape) == (4, 1, spec["llama"]["vocab_size"]) and out.loss is None
+    sd = H.bf16_round(weights)
+    o = O.forward(inp, sd, hp, dtype=torch.float32)
+    ob = O.forward(inp, sd, hp, dtype=torch.bfloat16)
+    e_log = H.rel_err(out.logits.cpu(), o["logits"])
+    r_log = H.rel_err(ob["logits"], o["logits"])
+    print(f"\n[parity:T=1] logits {e_log:.3e} | reference algorithm in bf16: logits {r_log:.3e}")
+    assert e_log < 1e-2 and e_log < 2.0 * max(r_log, 2e-3)
+
+
 def test_encoders_vs_oracle(tiny):
     from oracle import macaw_oracle as O
 

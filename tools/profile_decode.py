@@ -18,7 +18,6 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--new", type=int, default=32)
-    ap.add_argument("--fused", type=int, default=1, help="0: the unfused decode tails (thin_reduce + rope_rows + kv_append ...)")
     args = ap.parse_args()
     import bench
     from macaw_llm_b200.modeling import MM_LLMs, MM_LLMs_Config
@@ -29,7 +28,6 @@ def main():
     V, B, L = llama.vocab_size, 8, 256
     cfg = MM_LLMs_Config(clip_config=clip, whisper_config=whisper, llm_config=llama, **hyper)
     model = MM_LLMs.build_random(cfg, device=dev, dtype=torch.bfloat16, seed=0)
-    model.engine.fused_decode_tails = bool(args.fused)
     host = bench.synth_inputs(B, L, V, clip.vision_config.image_size, 2 * whisper.max_source_positions, 1234)
     inp = {k: (v.to(dev) if isinstance(v, torch.Tensor) else v) for k, v in host.items()}
     inp["audios"] = None
