@@ -155,8 +155,9 @@ int32_t mm_gemm_plan(const mm_gemm_args* args, mm_gemm_schedule* plan);
  * MACAW_B200_GEMM_STREAMK), 2 whenever the schedule allows (tests).  mode < 0 only queries.  Returns the previous mode. */
 int32_t mm_gemm_streamk_mode(int32_t mode);
 /* Epilogue-overlap policy of the process: 0 the consumer warpgroups run each tile's epilogue themselves, 1 a dedicated
- * epilogue warpgroup runs it while they start the next tile (default; environment MACAW_B200_GEMM_OVERLAP).  Outputs are
- * bit-identical in both modes.  mode < 0 only queries.  Returns the previous mode. */
+ * epilogue warpgroup runs it while they start the next tile, 2 as 1 and launches whose 128-wide N tiles pair up walk
+ * them two at a time under one 128 x 256 main loop (default; environment MACAW_B200_GEMM_OVERLAP).  Outputs are
+ * bit-identical in all modes.  mode < 0 only queries.  Returns the previous mode. */
 int32_t mm_gemm_overlap_mode(int32_t mode);
 /* bytes of mm_gemm_args.sk_workspace on the current device */
 int64_t mm_gemm_streamk_workspace_bytes(void);

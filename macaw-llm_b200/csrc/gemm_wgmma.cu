@@ -17,6 +17,9 @@
 // round-robin tile schedule with grouped rasterisation for L2 reuse.  A partial last wave can be split along K over all
 // CTAs (stream-K tail, gemm_work()).
 //
+// Launches of the epilogue-warpgroup kind whose 128-wide N tiles pair up run gemm_wide_kernel instead (overlap mode 2, the
+// default): the same tiles and epilogue, two N-neighbours per 128 x 256 x 64 main loop.  See the comment above it.
+//
 // Thin problems (decode steps) are launched with the operands swapped and `c_trans` set: the weight matrix takes the
 // 128-row A side, the few activation rows the narrow B side, and the standard epilogue stores transposed.
 //
@@ -784,6 +787,187 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 }
 
+// ------------------------------------------------------------------------------------------------ wide main loop
+// The same 128 x 128 output tiles, walked two N-neighbours at a time under one 128 x 256 x 64 main loop (m64n256k16 per
+// consumer warpgroup).  Per 64-deep k-block a 128 x 128 stage moves 80 KiB through shared memory (32 KiB written by TMA,
+// 2 x (8 + 16) KiB read by the two warpgroups) for 512 tensor-core cycles; the pair moves 128 KiB (48 written, 2 x (8 + 32)
+// read) for 1024, so A is fetched and read once for two tiles.  Everything that decides a value is unchanged: the k-order
+// of the MMAs, the accumulator fragment of each tile (acc[0..63] is the left tile in the n128 layout, acc[64..127] the
+// right one) and gemm_epilogue<128, EPI> itself, which the epilogue warpgroup runs once per tile of the pair.  Outputs are
+// therefore bit-identical to gemm_bf16_kernel<128, ...>.
+//
+// The staging tile holds one 128 x 128 tile, so the consumers hand the left tile over, wait until the epilogue warpgroup
+// has read it, hand the right one over and start the next pair; that one epilogue is exposed once per pair.
+//
+// 384 threads, not 512: one m64n256k16 needs its 128 accumulators plus operands in registers, and ptxas refuses the
+// instruction under the 128-register ceiling of a 512-thread block (168 at 384).  So there is no producer warpgroup: one
+// lane of consumer warp 0 issues the TMA loads, each into the ring slot the consumers have just released, which keeps
+// kWideStages - 1 k-blocks in flight across pair boundaries and through the hand-over.
+constexpr int kWideThreads = 384;
+constexpr int kWideStages = 3;
+constexpr uint32_t kWideBBytes = 2 * kMaxBN * kBlockK * 2;  // two 128-row B boxes = the 256-row K-major operand
+constexpr size_t kWideSmemBytes =
+    1024 + kWideStages * (kABytes + kWideBBytes) + (size_t)kBlockM * gemm_stage_ld(kMaxBN) * 4 + 256;
+static_assert(kWideSmemBytes <= 227 * 1024, "wide GEMM: ring + staging tile exceed an sm_90 block's shared memory");
+// setmaxnreg budgets of the three warpgroups (the block starts with 168 registers per thread)
+constexpr int kWideRegsConsumer = 184, kWideRegsEpilogue = 136;
+static_assert(2 * kWideRegsConsumer + kWideRegsEpilogue <= 3 * 168, "wide GEMM: register budget");
+
+// tile_coord() with N counted in pairs: work unit idx -> the left tile (m_blk, 2 j) of the pair
+__device__ __forceinline__ TileCoord pair_coord(int idx, const GemmKParams& p) {
+  const int n_pairs = p.n_tiles / 2;
+  const int in_group = p.group_m * n_pairs;
+  const int g = idx / in_group;
+  const int first_m = g * p.group_m;
+  const int gsz = min(p.m_tiles - first_m, p.group_m);
+  const int rr = idx - g * in_group;
+  TileCoord t;
+  t.b = t.b_lo = t.b_hi = 0;
+  t.m_blk = first_m + rr % gsz;
+  t.n_blk = 2 * (rr / gsz);
+  return t;
+}
+
+// K-major A and B, no batching, no stream-K tail, an even number of 128-wide N tiles (gemm_dispatch checks).
+template <int EPI, bool F16>
+__global__ void __launch_bounds__(kWideThreads, 1)
+gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmKParams p) {
+  constexpr int BN = kMaxBN;
+  constexpr int LDS = gemm_stage_ld(BN);
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sA = smem;
+  uint8_t* sB = smem + kWideStages * kABytes;
+  float* sC = reinterpret_cast<float*>(sB + kWideStages * kWideBBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sC + kBlockM * LDS);
+  uint64_t* empty_bar = full_bar + kWideStages;
+  uint64_t* staging_full = empty_bar + kWideStages;
+  uint64_t* staging_empty = staging_full + 1;
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int worker = static_cast<int>(blockIdx.x);
+  const int n_workers = static_cast<int>(gridDim.x);
+  const int total_pairs = p.m_tiles * (p.n_tiles / 2);
+
+  if (warp == 0 && elect_one()) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int s = 0; s < kWideStages; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);
+    }
+    mbar_init(staging_full, 256);
+    mbar_init(staging_empty, 128);
+    fence_mbar_init();
+  }
+  __syncthreads();
+  griddep_launch();
+  griddep_wait();
+
+  const int q = warp & 3;
+  if (warp >= 8) {
+    // ------------------------------------------------------------------ epilogue warpgroup: the pair's two tiles in turn
+    setmaxnreg_dec<kWideRegsEpilogue>();
+    const float* srow = sC + (q * 32 + lane) * LDS;
+    GemmWork wk;
+    wk.tile = 0; wk.kb0 = 0; wk.kb1 = p.num_k; wk.role = 0; wk.c0 = 0; wk.nc = 0;  // whole tiles only
+    for (int u = worker; u < total_pairs; u += n_workers) {
+      TileCoord t = pair_coord(u, p);
+      const float rs = epi_row_scale(p, t, t.m_blk * kBlockM + q * 32 + lane);  // one row statistic serves both tiles
+#pragma unroll 1
+      for (int side = 0; side < 2; ++side) {
+        mbar_wait(staging_full, side);  // two hand-overs per pair: the barrier's phase parity is the side
+        for (int half = 0; half < 2; ++half)
+          gemm_epilogue<BN, EPI>(p, t, wk, srow, rs, q, lane, half, q + 4 * half, worker, n_workers);
+        mbar_arrive(staging_empty);
+        ++t.n_blk;
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers
+  setmaxnreg_inc<kWideRegsConsumer>();
+  const int wg = warp >> 2;
+  int stage = 0;
+  uint32_t phase = 0;
+  // TMA loads, thread 0 only: the k-blocks of this CTA's pairs in order, each into the next ring slot once every
+  // consumer warp has released it (at once for the first kWideStages)
+  const bool loader = threadIdx.x == 0;
+  int ld_u = worker, ld_kb = 0, ld_stage = 0;
+  uint32_t ld_phase = 0;
+  TileCoord ld_t = pair_coord(worker, p);
+  auto load_next = [&]() {
+    if (ld_u >= total_pairs) return;
+    mbar_wait(&empty_bar[ld_stage], ld_phase ^ 1);
+    mbar_arrive_expect_tx(&full_bar[ld_stage], kABytes + kWideBBytes);
+    tma_load_4d(&tmA, &full_bar[ld_stage], sA + ld_stage * kABytes, ld_kb * kBlockK, ld_t.m_blk * kBlockM, 0, 0);
+    uint8_t* b = sB + ld_stage * kWideBBytes;
+    tma_load_4d(&tmB, &full_bar[ld_stage], b, ld_kb * kBlockK, ld_t.n_blk * BN, 0, 0);
+    tma_load_4d(&tmB, &full_bar[ld_stage], b + kWideBBytes / 2, ld_kb * kBlockK, (ld_t.n_blk + 1) * BN, 0, 0);
+    if (++ld_stage == kWideStages) {
+      ld_stage = 0;
+      ld_phase ^= 1;
+    }
+    if (++ld_kb == p.num_k) {
+      ld_kb = 0;
+      ld_u += n_workers;
+      if (ld_u < total_pairs) ld_t = pair_coord(ld_u, p);
+    }
+  };
+  if (loader)
+    for (int s = 0; s < kWideStages; ++s) load_next();
+  __syncwarp();
+  for (int u = worker; u < total_pairs; u += n_workers) {
+    float acc[2 * BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN; ++i) acc[i] = 0.f;
+    int prev = -1;
+    for (int kb = 0; kb < p.num_k; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint64_t a_desc = make_sdesc_sw128(smem_u32(sA + stage * kABytes) + wg * 8192, 16, 1024);
+      const uint64_t b_desc = make_sdesc_sw128(smem_u32(sB + stage * kWideBBytes), 16, 1024);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < kBlockK / 16; ++kk)
+        wgmma_ss_n256<F16, 0, 0>(acc, a_desc + static_cast<uint64_t>(kk * 2), b_desc + static_cast<uint64_t>(kk * 2), 1u);
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous k-block's MMAs have retired: its smem slot is free
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        if (loader) load_next();
+        __syncwarp();
+      }
+      prev = stage;
+      if (++stage == kWideStages) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    fence_regs(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    if (loader) load_next();
+    __syncwarp();
+    const int r0 = wg * 64 + q * 16 + (lane >> 2);
+    const int c0 = 2 * (lane & 3);
+#pragma unroll
+    for (int side = 0; side < 2; ++side) {
+      mbar_wait(staging_empty, side ^ 1);  // the previous hand-over has been read (passes at once for the first)
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int i = side * (BN / 2) + 4 * j;
+        *reinterpret_cast<float2*>(sC + r0 * LDS + 8 * j + c0) = make_float2(acc[i], acc[i + 1]);
+        *reinterpret_cast<float2*>(sC + (r0 + 8) * LDS + 8 * j + c0) = make_float2(acc[i + 2], acc[i + 3]);
+      }
+      mbar_arrive(staging_full);
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -836,9 +1020,9 @@ static int& streamk_mode() {
   return mode;
 }
 
-// process-wide epilogue-overlap policy; initial value from MACAW_B200_GEMM_OVERLAP (default 1)
+// process-wide epilogue-overlap policy; initial value from MACAW_B200_GEMM_OVERLAP (default 2)
 static int& overlap_mode() {
-  static int mode = []() { const char* e = getenv("MACAW_B200_GEMM_OVERLAP"); const int v = e ? atoi(e) : 1; return v < 0 || v > 1 ? 1 : v; }();
+  static int mode = []() { const char* e = getenv("MACAW_B200_GEMM_OVERLAP"); const int v = e ? atoi(e) : 2; return v < 0 || v > 2 ? 2 : v; }();
   return mode;
 }
 
@@ -857,6 +1041,21 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmK
   const int total = p.batch * p.batch2 * p.m_tiles * p.n_tiles;
   const int grid = (total < num_sms() && p.sk_tiles == 0) ? total : num_sms();  // stream-K shares the tail over ALL SMs
   cudaError_t e = launch_kernel(kern, dim3(grid), dim3(ewg ? kGemmThreadsEwg : kGemmThreads), smem, st, 1, ta, tb, p);
+  if (e != cudaSuccess) {
+    set_error("mm_gemm_fwd: launch failed: %s", cudaGetErrorString(e));
+    return 2;
+  }
+  return check_launch("mm_gemm_fwd");
+}
+
+template <int EPI>
+static int launch_gemm_wide(const CUtensorMap& ta, const CUtensorMap& tb, const GemmKParams& p, bool f16, cudaStream_t st) {
+  static bool attr_set[2][kMaxDevices] = {};
+  auto kern = f16 ? gemm_wide_kernel<EPI, true> : gemm_wide_kernel<EPI, false>;
+  if (int rc = ensure_smem_attr(kern, kWideSmemBytes, attr_set[f16 ? 1 : 0], "mm_gemm_fwd")) return rc;
+  const int pairs = p.m_tiles * (p.n_tiles / 2);
+  cudaError_t e = launch_kernel(kern, dim3(pairs < num_sms() ? pairs : num_sms()), dim3(kWideThreads), kWideSmemBytes,
+                                st, 1, ta, tb, p);
   if (e != cudaSuccess) {
     set_error("mm_gemm_fwd: launch failed: %s", cudaGetErrorString(e));
     return 2;
@@ -940,7 +1139,11 @@ static int32_t gemm_dispatch(const mm_gemm_args* a, void* stream, mm_gemm_schedu
   } else {
     // Cost model (cycles per 64-deep k-block of one tile; two warpgroups of m64nBNk16): the tensor cores need 4 BN cycles
     // (2048 dense bf16 FMA per cycle and SM), shared memory must deliver each warpgroup's 8 KiB of A plus the whole B
-    // tile (128 BN bytes) at 128 B/cycle -> 128 + 2 BN cycles.  BN = 64 sits on both limits (10 % penalty).
+    // tile (128 BN bytes) at 128 B/cycle -> 128 + 2 BN cycles.  BN = 64 sits on both limits (10 % penalty).  The model
+    // counts the operand reads only: TMA also WRITES the stage (16 KiB + 128 BN bytes) through the same shared memory,
+    // which adds 128 + BN cycles if it is charged in full -> 640 at BN = 128, above the tensor cores' 512 (the measured
+    // main loop, profiles/h100_gemm_schedule.txt, sits nearer 640 than 512).  The ranking of the three widths is the
+    // same either way; the wide kernel of mode 2 exists because of that write traffic.
     // Waves = ceil(tiles / SMs).
     const int cands[3] = {128, 64, 32};
     const long long kcost[3] = {512, 282, 192};
@@ -1027,7 +1230,16 @@ static int32_t gemm_dispatch(const mm_gemm_args* a, void* stream, mm_gemm_schedu
   const bool f16 = a->a_fp16 != 0;
   // A stream-K launch keeps the consumer epilogue: the epilogue warpgroup handles whole tiles only (the tail's pieces of
   // one or two k-blocks would leave it nothing to overlap).
-  const bool ewg = overlap_mode() == 1 && p.num_k >= kEwgMinKBlocks && p.sk_tiles == 0;
+  const bool ewg = overlap_mode() >= 1 && p.num_k >= kEwgMinKBlocks && p.sk_tiles == 0;
+  // Mode 2: launches that the epilogue warpgroup would take, whose 128-wide N tiles pair up without a remainder and fill
+  // at least one wave of pairs, walk those tiles two at a time (gemm_wide_kernel).  The plan above is unchanged: same
+  // tiles, same epilogue, same bits.
+  if (overlap_mode() == 2 && ewg && BN == kMaxBN && !a->a_mn_major && !a->b_mn_major && !a->c_trans && a->batch == 1 &&
+      batch2 == 1 && p.n_tiles % 2 == 0 && tiles / 2 >= sms) {
+    if (a->epi == MM_EPI_ROPE) return launch_gemm_wide<MM_EPI_ROPE>(ta, tb, p, f16, st);
+    if (a->epi == MM_EPI_SWIGLU) return launch_gemm_wide<MM_EPI_SWIGLU>(ta, tb, p, f16, st);
+    return launch_gemm_wide<MM_EPI_STD>(ta, tb, p, f16, st);
+  }
 
 #define MM_LAUNCH(BN_, EPI_, MN_) return launch_gemm<BN_, EPI_, MN_>(ta, tb, p, f16, ewg, st)
   if (a->epi == MM_EPI_ROPE) MM_LAUNCH(128, MM_EPI_ROPE, false);
@@ -1061,7 +1273,7 @@ extern "C" int32_t mm_gemm_streamk_mode(int32_t mode) {
 
 extern "C" int32_t mm_gemm_overlap_mode(int32_t mode) {
   const int prev = overlap_mode();
-  if (mode >= 0 && mode <= 1) overlap_mode() = mode;
+  if (mode >= 0 && mode <= 2) overlap_mode() = mode;
   return prev;
 }
 

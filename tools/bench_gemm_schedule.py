@@ -3,6 +3,9 @@
 
   python tools/bench_gemm_schedule.py [--modes 0,1] [--rounds 3] [--iters 20] [--dtype fp16] [--out FILE]
 
+Modes: 0 consumer epilogue, 1 epilogue warpgroup, 2 epilogue warpgroup + the 128 x 256 main loop for launches whose N
+tiles pair up (the LLaMA and lm_head rows, CLIP / Whisper fc2, the K sweep from K = 2048); e.g. `--modes 1,2`.
+
 Two tables; every measurement is repeated once per mode for `--rounds` rounds, and per GEMM the modes alternate within
 each round, in swapped order every other round (median and min..max reported):
   K sweep   M = 16896, N = 4096, the o_proj epilogue (residual + sumsq_out), K in {512 .. 8192}.  Time per tile of one CTA
@@ -73,7 +76,7 @@ def card():
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--modes", default="0,1")
+    ap.add_argument("--modes", default="0,1", help="comma-separated overlap modes out of 0, 1, 2")
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--dtype", default="fp16", choices=["bf16", "fp16"])
@@ -82,6 +85,7 @@ def main():
     from macaw_llm_b200 import _lib, ops
 
     modes = [int(m) for m in a.modes.split(",")]
+    assert modes and all(m in (0, 1, 2) for m in modes), "--modes takes overlap modes 0, 1 and 2"
     lib = _lib.load()
     dt = torch.float16 if a.dtype == "fp16" else torch.bfloat16
     ops.set_act_format(dt)
