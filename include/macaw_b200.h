@@ -133,17 +133,25 @@ typedef struct mm_gemm_args {
 
 int32_t mm_gemm_fwd(const mm_gemm_args* args, void* stream);
 /* The schedule mm_gemm_fwd would use for `args` on the current device (132 SMs when no device is visible), without
- * touching memory or launching: the host-side decisions — tile width from the cost model,
- * rasterisation group, stream-K tail — are a pure function of the shapes, strides, alignments and flags.  Operand
- * pointers are only checked for null / alignment, never dereferenced.  Host logic made testable without a GPU
- * (tests/test_gemm_plan.py) and printable per BASELINE shape (tools/gemm_plan.py). */
+ * touching memory or launching: the host-side decisions — tile width from the cost model, rasterisation group,
+ * stream-K tail, kernel variant and launch shape — are a pure function of the shapes, strides, alignments and flags.
+ * Operand pointers are only checked for null / alignment, never dereferenced.  Host logic made testable without a GPU
+ * (tests/test_gemm_plan.py) and printable per BASELINE shape (tools/gemm_plan.py).
+ * m_tiles, n_tiles, units and waves describe the 128 x block_n tile grid whichever kernel runs it; kernel, threads,
+ * grid and smem_bytes describe the launch itself (a TILE_PAIRS CTA takes two N-neighbouring tiles at a time). */
+enum {
+  MM_GEMM_KERNEL_CONSUMER_EPILOGUE = 0,  /* 288 threads: the consumer warpgroups run each tile's epilogue */
+  MM_GEMM_KERNEL_EPILOGUE_WARPGROUP = 1, /* 512 threads: a dedicated epilogue warpgroup (mm_gemm_overlap_mode 1, 2) */
+  MM_GEMM_KERNEL_TILE_PAIRS = 2          /* 384 threads: two 128-wide tiles per 128 x 256 main loop (mode 2) */
+};
 typedef struct mm_gemm_schedule {
   int32_t block_n;             /* tile = 128 x block_n x 64 */
-  int32_t pairs;               /* always 0: every tile runs on one CTA (no CTA-pair schedules on sm_90a) */
+  int32_t kernel;              /* MM_GEMM_KERNEL_*: the kernel variant launched */
   int32_t m_tiles, n_tiles, k_blocks;
   int64_t units;               /* work units over all batches: tiles */
   int32_t workers;             /* units in flight: SMs */
   int32_t grid;                /* CTAs launched (persistent: <= SM count) */
+  int32_t threads;             /* threads per CTA */
   int32_t waves;               /* ceil(units / workers) */
   int32_t group_m;             /* rasterisation: M units per L2 group */
   int32_t streamk_tiles;       /* tiles of the partial last wave shared over all CTAs (0 = plain tiles) */

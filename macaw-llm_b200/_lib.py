@@ -37,9 +37,9 @@ class GemmArgs(C.Structure):
 class GemmPlan(C.Structure):
     """Mirror of `mm_gemm_schedule` (include/macaw_b200.h), filled by mm_gemm_plan()."""
 
-    _fields_ = [("block_n", c_i32), ("pairs", c_i32), ("m_tiles", c_i32), ("n_tiles", c_i32), ("k_blocks", c_i32),
-                ("units", c_i64), ("workers", c_i32), ("grid", c_i32), ("waves", c_i32), ("group_m", c_i32),
-                ("streamk_tiles", c_i32), ("smem_bytes", c_i32), ("vectorised_epilogue", c_i32)]
+    _fields_ = [("block_n", c_i32), ("kernel", c_i32), ("m_tiles", c_i32), ("n_tiles", c_i32), ("k_blocks", c_i32),
+                ("units", c_i64), ("workers", c_i32), ("grid", c_i32), ("threads", c_i32), ("waves", c_i32),
+                ("group_m", c_i32), ("streamk_tiles", c_i32), ("smem_bytes", c_i32), ("vectorised_epilogue", c_i32)]
 
 
 class ThinArgs(C.Structure):
@@ -172,7 +172,7 @@ SIGNATURES = {
 NULLABLE_BEFORE_STREAM = {"mm_adamw": 1, "mm_adamw_host": 1}
 
 _lib = None
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 
 class _NullableBeforeStream:

@@ -41,7 +41,7 @@ int num_sms() {
 
 extern "C" {
 const char* mm_last_error(void) { return mm::g_err; }
-int32_t mm_abi_version(void) { return 7; }
+int32_t mm_abi_version(void) { return 8; }
 #ifndef MM_SRC_HASH
 #define MM_SRC_HASH "unknown"
 #endif

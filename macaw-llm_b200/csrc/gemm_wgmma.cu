@@ -4,7 +4,7 @@
 //   warps 0..7  : two consumer warpgroups; warpgroup g issues wgmma for rows 64 g .. 64 g + 63 of the tile (accumulators
 //                 in registers), then all eight warps run the epilogue (bias/activation/residual/RoPE/SwiGLU -> global)
 //
-// With EWG (epilogue warpgroup, 512 threads: long-K launches without a stream-K tail, see gemm_dispatch) the epilogue has warpgroup 2 (warps 8..11)
+// With EWG (epilogue warpgroup, 512 threads: long-K launches without a stream-K tail, see plan_gemm) the epilogue has warpgroup 2 (warps 8..11)
 // to itself and the producer moves to warp 12 (warpgroup 3); setmaxnreg gives the registers the producer warpgroup does
 // not need to the others (40 / 152 / 168).  A consumer warpgroup waits on `staging_empty`, stores its accumulators to the
 // staging tile, arrives on `staging_full` and starts the next tile's main loop at once; the epilogue warpgroup waits on
@@ -90,9 +90,42 @@ __host__ __device__ constexpr int gemm_stages(int BN) {
   return BN >= 128 ? 4 : (BN >= 64 ? 6 : 8);
 }
 __host__ __device__ constexpr int gemm_stage_ld(int BN) { return BN + 4; }  // staging row stride (floats): conflict-free row reads
-__host__ __device__ constexpr size_t gemm_smem_bytes(int BN) {
-  return 1024 /*align slack*/ + (size_t)gemm_stages(BN) * (kABytes + BN * kBlockK * 2) +
-         (size_t)kBlockM * gemm_stage_ld(BN) * 4 + 256 /*barriers*/;
+// Dynamic shared memory of a GEMM CTA (the layout of gemm_smem()): a ring of `stages` A and B stages, the fp32 staging
+// tile of one 128 x BN tile and the barriers.
+__host__ __device__ constexpr size_t gemm_smem_bytes(int stages, uint32_t b_bytes, int BN) {
+  return 1024 /*align slack*/ + (size_t)stages * (kABytes + b_bytes) + (size_t)kBlockM * gemm_stage_ld(BN) * 4 +
+         256 /*barriers*/;
+}
+
+// sC: the staging tile, row stride gemm_stage_ld(BN).  With an epilogue warpgroup, staging_full = the consumers have
+// written a tile's accumulators to sC, staging_empty = the epilogue warpgroup is done with sC.
+struct GemmSmem {
+  uint8_t *sA, *sB;
+  float* sC;
+  uint64_t *full_bar, *empty_bar, *staging_full, *staging_empty;
+};
+template <int STAGES, uint32_t B_BYTES, int BN>
+__device__ __forceinline__ GemmSmem gemm_smem(uint8_t* smem_raw) {
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sB = smem + STAGES * kABytes;
+  float* sC = reinterpret_cast<float*>(sB + STAGES * B_BYTES);
+  uint64_t* bar = reinterpret_cast<uint64_t*>(sC + kBlockM * gemm_stage_ld(BN));
+  return {smem, sB, sC, bar, bar + STAGES, bar + 2 * STAGES, bar + 2 * STAGES + 1};
+}
+// Run by one elected thread before the block's __syncthreads(): descriptor prefetch and barrier initialisation.
+template <int STAGES, bool STAGING>
+__device__ __forceinline__ void gemm_prologue(const GemmSmem& s, const CUtensorMap* tmA, const CUtensorMap* tmB) {
+  tma_prefetch_desc(tmA);
+  tma_prefetch_desc(tmB);
+  for (int i = 0; i < STAGES; ++i) {
+    mbar_init(&s.full_bar[i], 1);
+    mbar_init(&s.empty_bar[i], 8);  // one arrival per consumer warp
+  }
+  if constexpr (STAGING) {
+    mbar_init(s.staging_full, 256);  // every consumer thread, after its accumulator stores
+    mbar_init(s.staging_empty, 128);  // every epilogue thread, after its last staging read
+  }
+  fence_mbar_init();
 }
 
 struct TileCoord {
@@ -613,6 +646,33 @@ __device__ __forceinline__ void gemm_epilogue(const GemmKParams& p, const TileCo
   }
 }
 
+// Store one BN-wide tile of this thread's accumulator fragment (m64nBNk16 layout, acc[off .. off + BN / 2)) to rows
+// wg * 64 .. wg * 64 + 63 of the staging tile.
+template <int BN, int N>
+__device__ __forceinline__ void stage_acc(float* sC, const float (&acc)[N], int off, int wg, int q, int lane) {
+  constexpr int LDS = gemm_stage_ld(BN);
+  const int r0 = wg * 64 + q * 16 + (lane >> 2);
+  const int c0 = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int i = off + 4 * j;
+    *reinterpret_cast<float2*>(sC + r0 * LDS + 8 * j + c0) = make_float2(acc[i], acc[i + 1]);
+    *reinterpret_cast<float2*>(sC + (r0 + 8) * LDS + 8 * j + c0) = make_float2(acc[i + 2], acc[i + 3]);
+  }
+}
+
+// The epilogue warpgroup's turn on one whole tile: wait for the consumers' hand-over (phase `parity` of staging_full),
+// run the epilogue over both column halves of this thread's row of sC (srow; rs = epi_row_scale()), release sC.
+template <int BN, int EPI>
+__device__ __forceinline__ void ewg_tile(const GemmKParams& p, const GemmSmem& s, const TileCoord& t, const GemmWork& wk,
+                                         const float* srow, float rs, uint32_t parity, int q, int lane, int worker,
+                                         int n_workers) {
+  mbar_wait(s.staging_full, parity);
+  for (int half = 0; half < 2; ++half)
+    gemm_epilogue<BN, EPI>(p, t, wk, srow, rs, q, lane, half, q + 4 * half, worker, n_workers);
+  mbar_arrive(s.staging_empty);
+}
+
 // A_MN = true: A is given as [K][M] with M contiguous (the transpose of a row-major [tokens][features] activation): the
 // weight-gradient GEMM dW = dY^T X reads dY and X exactly as the forward pass wrote them, no transpose copies.
 // B_MN = true: B is given as [K][N] with N contiguous.  F16: IEEE half operands, else bf16.
@@ -628,14 +688,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   constexpr int LDS = gemm_stage_ld(BN);
 
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + STAGES * kABytes;
-  float* sC = reinterpret_cast<float*>(sB + STAGES * B_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sC + kBlockM * LDS);
-  uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* staging_full = empty_bar + STAGES;  // EWG: the consumers have written a tile's accumulators to sC
-  uint64_t* staging_empty = staging_full + 1;   // EWG: the epilogue warpgroup is done with sC
+  const GemmSmem sm = gemm_smem<STAGES, B_BYTES, BN>(smem_raw);
 
   constexpr int kProducer = EWG ? kProducerWarpEwg : kProducerWarp;
   const int warp = threadIdx.x >> 5;
@@ -645,19 +698,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int m_units = p.m_tiles;
   const int total_tiles = p.batch * p.batch2 * m_units * p.n_tiles;
 
-  if (warp == kProducer && elect_one()) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 8);  // one arrival per consumer warp
-    }
-    if constexpr (EWG) {
-      mbar_init(staging_full, 256);  // every consumer thread, after its accumulator stores
-      mbar_init(staging_empty, 128);  // every epilogue thread, after its last staging read
-    }
-    fence_mbar_init();
-  }
+  if (warp == kProducer && elect_one()) gemm_prologue<STAGES, EWG>(sm, &tmA, &tmB);
   __syncthreads();
   // prologue done (barriers, descriptors): let the next kernel start its own, then wait for our inputs
   griddep_launch();
@@ -675,22 +716,23 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const int bb = p.b_shared ? 0 : t.b_lo;
         const int bh = p.b2_shared ? 0 : t.b_hi;
         for (int kb = wk.kb0; kb < wk.kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full_bar[stage], kABytes + B_BYTES);
+          mbar_wait(&sm.empty_bar[stage], phase ^ 1);
+          mbar_arrive_expect_tx(&sm.full_bar[stage], kABytes + B_BYTES);
           if constexpr (A_MN) {
 #pragma unroll
             for (int j = 0; j < kBlockM / 64; ++j)
-              tma_load_4d(&tmA, &full_bar[stage], sA + stage * kABytes + j * 8192, t.m_blk * kBlockM + j * 64,
+              tma_load_4d(&tmA, &sm.full_bar[stage], sm.sA + stage * kABytes + j * 8192, t.m_blk * kBlockM + j * 64,
                           kb * kBlockK, t.b_lo, t.b_hi);
           } else {
-            tma_load_4d(&tmA, &full_bar[stage], sA + stage * kABytes, kb * kBlockK, t.m_blk * kBlockM, t.b_lo, t.b_hi);
+            tma_load_4d(&tmA, &sm.full_bar[stage], sm.sA + stage * kABytes, kb * kBlockK, t.m_blk * kBlockM, t.b_lo,
+                        t.b_hi);
           }
           if constexpr (!B_MN) {
-            tma_load_4d(&tmB, &full_bar[stage], sB + stage * B_BYTES, kb * kBlockK, t.n_blk * BN, bb, bh);
+            tma_load_4d(&tmB, &sm.full_bar[stage], sm.sB + stage * B_BYTES, kb * kBlockK, t.n_blk * BN, bb, bh);
           } else {
 #pragma unroll
             for (int j = 0; j < BN / 64; ++j)
-              tma_load_4d(&tmB, &full_bar[stage], sB + stage * B_BYTES + j * 8192, t.n_blk * BN + j * 64,
+              tma_load_4d(&tmB, &sm.full_bar[stage], sm.sB + stage * B_BYTES + j * 8192, t.n_blk * BN + j * 64,
                           kb * kBlockK, bb, bh);
           }
           if (++stage == STAGES) {
@@ -704,20 +746,18 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 
   const int q = warp & 3;  // the epilogue rows of this warp: q * 32 + lane
-  const float* srow = sC + (q * 32 + lane) * LDS;
+  const float* srow = sm.sC + (q * 32 + lane) * LDS;
   if (EWG && warp >= 8) {
     // ------------------------------------------------------------------ epilogue warpgroup: every column of its rows
     if constexpr (EWG) setmaxnreg_inc<168>();
     GemmWork wk;
-    // EWG launches have no stream-K tail (launch_gemm refuses one): every work unit is a whole tile (role 0), so the
-    // stream-K flag lane passed below is never used
+    // EWG launches have no stream-K tail (the launch plan never pairs them): every work unit is a whole tile (role 0),
+    // so the stream-K flag lane passed below is never used
     for (int it = 0; gemm_work(p, worker, n_workers, total_tiles, it, wk); ++it) {
       const TileCoord t = tile_coord(wk.tile, p, m_units);
       // the row statistic's L2 reads are issued before the wait: they overlap the tile's main loop
       const float rs = epi_row_scale(p, t, t.m_blk * kBlockM + q * 32 + lane);
-      mbar_wait(staging_full, it & 1);
-      for (int half = 0; half < 2; ++half) gemm_epilogue<BN, EPI>(p, t, wk, srow, rs, q, lane, half, q + 4 * half, worker, n_workers);
-      mbar_arrive(staging_empty);
+      ewg_tile<BN, EPI>(p, sm, t, wk, srow, rs, it & 1, q, lane, worker, n_workers);
     }
     return;
   }
@@ -736,10 +776,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       int prev = -1;
       for (int kb = wk.kb0; kb < wk.kb1; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
+        mbar_wait(&sm.full_bar[stage], phase);
         // this warpgroup's 64 rows: +8 KiB in both A layouts (K-major rows of 128 B | the second 64-row MN block)
-        const uint32_t a_addr = smem_u32(sA + stage * kABytes) + wg * 8192;
-        const uint32_t b_addr = smem_u32(sB + stage * B_BYTES);
+        const uint32_t a_addr = smem_u32(sm.sA + stage * kABytes) + wg * 8192;
+        const uint32_t b_addr = smem_u32(sm.sB + stage * B_BYTES);
         const uint64_t a_desc = make_sdesc_sw128(a_addr, A_MN ? 8192 : 16, 1024);
         const uint64_t b_desc = make_sdesc_sw128(b_addr, B_MN ? 8192 : 16, 1024);
         wgmma_fence();
@@ -751,7 +791,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         wgmma_wait<1>();  // the previous k-block's MMAs have retired: its smem slot is free
         if (prev >= 0) {
           __syncwarp();
-          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+          if (lane == 0) mbar_arrive(&sm.empty_bar[prev]);
         }
         prev = stage;
         if (++stage == STAGES) {
@@ -762,19 +802,13 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       wgmma_wait<0>();
       fence_regs(acc);
       __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      if (lane == 0) mbar_arrive(&sm.empty_bar[prev]);
       // accumulators -> staging tile (the previous tile's epilogue must be done reading it)
-      if constexpr (EWG) mbar_wait(staging_empty, (it & 1) ^ 1);
+      if constexpr (EWG) mbar_wait(sm.staging_empty, (it & 1) ^ 1);
       else consumer_sync();
-      const int r0 = wg * 64 + q * 16 + (lane >> 2);
-      const int c0 = 2 * (lane & 3);
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        *reinterpret_cast<float2*>(sC + r0 * LDS + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
-        *reinterpret_cast<float2*>(sC + (r0 + 8) * LDS + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-      }
+      stage_acc<BN>(sm.sC, acc, 0, wg, q, lane);
       if constexpr (EWG) {
-        mbar_arrive(staging_full);
+        mbar_arrive(sm.staging_full);
         continue;  // straight on to the next tile's main loop
       }
       consumer_sync();
@@ -806,8 +840,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 constexpr int kWideThreads = 384;
 constexpr int kWideStages = 3;
 constexpr uint32_t kWideBBytes = 2 * kMaxBN * kBlockK * 2;  // two 128-row B boxes = the 256-row K-major operand
-constexpr size_t kWideSmemBytes =
-    1024 + kWideStages * (kABytes + kWideBBytes) + (size_t)kBlockM * gemm_stage_ld(kMaxBN) * 4 + 256;
+constexpr size_t kWideSmemBytes = gemm_smem_bytes(kWideStages, kWideBBytes, kMaxBN);
 static_assert(kWideSmemBytes <= 227 * 1024, "wide GEMM: ring + staging tile exceed an sm_90 block's shared memory");
 // setmaxnreg budgets of the three warpgroups (the block starts with 168 registers per thread)
 constexpr int kWideRegsConsumer = 184, kWideRegsEpilogue = 136;
@@ -828,21 +861,13 @@ __device__ __forceinline__ TileCoord pair_coord(int idx, const GemmKParams& p) {
   return t;
 }
 
-// K-major A and B, no batching, no stream-K tail, an even number of 128-wide N tiles (gemm_dispatch checks).
+// K-major A and B, no batching, no stream-K tail, an even number of 128-wide N tiles (the launch plan's conditions).
 template <int EPI, bool F16>
 __global__ void __launch_bounds__(kWideThreads, 1)
 gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmKParams p) {
   constexpr int BN = kMaxBN;
-  constexpr int LDS = gemm_stage_ld(BN);
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + kWideStages * kABytes;
-  float* sC = reinterpret_cast<float*>(sB + kWideStages * kWideBBytes);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sC + kBlockM * LDS);
-  uint64_t* empty_bar = full_bar + kWideStages;
-  uint64_t* staging_full = empty_bar + kWideStages;
-  uint64_t* staging_empty = staging_full + 1;
+  const GemmSmem sm = gemm_smem<kWideStages, kWideBBytes, BN>(smem_raw);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -850,17 +875,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int n_workers = static_cast<int>(gridDim.x);
   const int total_pairs = p.m_tiles * (p.n_tiles / 2);
 
-  if (warp == 0 && elect_one()) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int s = 0; s < kWideStages; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 8);
-    }
-    mbar_init(staging_full, 256);
-    mbar_init(staging_empty, 128);
-    fence_mbar_init();
-  }
+  if (warp == 0 && elect_one()) gemm_prologue<kWideStages, true>(sm, &tmA, &tmB);
   __syncthreads();
   griddep_launch();
   griddep_wait();
@@ -869,7 +884,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (warp >= 8) {
     // ------------------------------------------------------------------ epilogue warpgroup: the pair's two tiles in turn
     setmaxnreg_dec<kWideRegsEpilogue>();
-    const float* srow = sC + (q * 32 + lane) * LDS;
+    const float* srow = sm.sC + (q * 32 + lane) * gemm_stage_ld(BN);
     GemmWork wk;
     wk.tile = 0; wk.kb0 = 0; wk.kb1 = p.num_k; wk.role = 0; wk.c0 = 0; wk.nc = 0;  // whole tiles only
     for (int u = worker; u < total_pairs; u += n_workers) {
@@ -877,10 +892,8 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const float rs = epi_row_scale(p, t, t.m_blk * kBlockM + q * 32 + lane);  // one row statistic serves both tiles
 #pragma unroll 1
       for (int side = 0; side < 2; ++side) {
-        mbar_wait(staging_full, side);  // two hand-overs per pair: the barrier's phase parity is the side
-        for (int half = 0; half < 2; ++half)
-          gemm_epilogue<BN, EPI>(p, t, wk, srow, rs, q, lane, half, q + 4 * half, worker, n_workers);
-        mbar_arrive(staging_empty);
+        // two hand-overs per pair: the barrier's phase parity is the side
+        ewg_tile<BN, EPI>(p, sm, t, wk, srow, rs, side, q, lane, worker, n_workers);
         ++t.n_blk;
       }
     }
@@ -900,12 +913,12 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   TileCoord ld_t = pair_coord(worker, p);
   auto load_next = [&]() {
     if (ld_u >= total_pairs) return;
-    mbar_wait(&empty_bar[ld_stage], ld_phase ^ 1);
-    mbar_arrive_expect_tx(&full_bar[ld_stage], kABytes + kWideBBytes);
-    tma_load_4d(&tmA, &full_bar[ld_stage], sA + ld_stage * kABytes, ld_kb * kBlockK, ld_t.m_blk * kBlockM, 0, 0);
-    uint8_t* b = sB + ld_stage * kWideBBytes;
-    tma_load_4d(&tmB, &full_bar[ld_stage], b, ld_kb * kBlockK, ld_t.n_blk * BN, 0, 0);
-    tma_load_4d(&tmB, &full_bar[ld_stage], b + kWideBBytes / 2, ld_kb * kBlockK, (ld_t.n_blk + 1) * BN, 0, 0);
+    mbar_wait(&sm.empty_bar[ld_stage], ld_phase ^ 1);
+    mbar_arrive_expect_tx(&sm.full_bar[ld_stage], kABytes + kWideBBytes);
+    tma_load_4d(&tmA, &sm.full_bar[ld_stage], sm.sA + ld_stage * kABytes, ld_kb * kBlockK, ld_t.m_blk * kBlockM, 0, 0);
+    uint8_t* b = sm.sB + ld_stage * kWideBBytes;
+    tma_load_4d(&tmB, &sm.full_bar[ld_stage], b, ld_kb * kBlockK, ld_t.n_blk * BN, 0, 0);
+    tma_load_4d(&tmB, &sm.full_bar[ld_stage], b + kWideBBytes / 2, ld_kb * kBlockK, (ld_t.n_blk + 1) * BN, 0, 0);
     if (++ld_stage == kWideStages) {
       ld_stage = 0;
       ld_phase ^= 1;
@@ -925,9 +938,9 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     for (int i = 0; i < BN; ++i) acc[i] = 0.f;
     int prev = -1;
     for (int kb = 0; kb < p.num_k; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint64_t a_desc = make_sdesc_sw128(smem_u32(sA + stage * kABytes) + wg * 8192, 16, 1024);
-      const uint64_t b_desc = make_sdesc_sw128(smem_u32(sB + stage * kWideBBytes), 16, 1024);
+      mbar_wait(&sm.full_bar[stage], phase);
+      const uint64_t a_desc = make_sdesc_sw128(smem_u32(sm.sA + stage * kABytes) + wg * 8192, 16, 1024);
+      const uint64_t b_desc = make_sdesc_sw128(smem_u32(sm.sB + stage * kWideBBytes), 16, 1024);
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < kBlockK / 16; ++kk)
@@ -936,7 +949,7 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       wgmma_wait<1>();  // the previous k-block's MMAs have retired: its smem slot is free
       if (prev >= 0) {
         __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        if (lane == 0) mbar_arrive(&sm.empty_bar[prev]);
         if (loader) load_next();
         __syncwarp();
       }
@@ -949,21 +962,14 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     wgmma_wait<0>();
     fence_regs(acc);
     __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+    if (lane == 0) mbar_arrive(&sm.empty_bar[prev]);
     if (loader) load_next();
     __syncwarp();
-    const int r0 = wg * 64 + q * 16 + (lane >> 2);
-    const int c0 = 2 * (lane & 3);
 #pragma unroll
     for (int side = 0; side < 2; ++side) {
-      mbar_wait(staging_empty, side ^ 1);  // the previous hand-over has been read (passes at once for the first)
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int i = side * (BN / 2) + 4 * j;
-        *reinterpret_cast<float2*>(sC + r0 * LDS + 8 * j + c0) = make_float2(acc[i], acc[i + 1]);
-        *reinterpret_cast<float2*>(sC + (r0 + 8) * LDS + 8 * j + c0) = make_float2(acc[i + 2], acc[i + 3]);
-      }
-      mbar_arrive(staging_full);
+      mbar_wait(sm.staging_empty, side ^ 1);  // the previous hand-over has been read (passes at once for the first)
+      stage_acc<BN>(sm.sC, acc, side * (BN / 2), wg, q, lane);
+      mbar_arrive(sm.staging_full);
     }
   }
 }
@@ -1026,51 +1032,17 @@ static int& overlap_mode() {
   return mode;
 }
 
-template <int BN, int EPI, bool B_MN, bool A_MN = false>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const GemmKParams& p, bool f16, bool ewg,
-                       cudaStream_t st) {
-  if (ewg && p.sk_tiles != 0) {  // the epilogue warpgroup implements whole tiles only (no stream-K hand-over)
-    set_error("mm_gemm_fwd: the epilogue-warpgroup kernel takes no stream-K tail");
-    return 1;
-  }
-  static bool attr_set[2][2][kMaxDevices] = {};
-  constexpr size_t smem = gemm_smem_bytes(BN);
-  auto kern = f16 ? (ewg ? gemm_bf16_kernel<BN, EPI, B_MN, A_MN, true, true> : gemm_bf16_kernel<BN, EPI, B_MN, A_MN, true, false>)
-                  : (ewg ? gemm_bf16_kernel<BN, EPI, B_MN, A_MN, false, true> : gemm_bf16_kernel<BN, EPI, B_MN, A_MN, false, false>);
-  if (int rc = ensure_smem_attr(kern, smem, attr_set[f16 ? 1 : 0][ewg ? 1 : 0], "mm_gemm_fwd")) return rc;
-  const int total = p.batch * p.batch2 * p.m_tiles * p.n_tiles;
-  const int grid = (total < num_sms() && p.sk_tiles == 0) ? total : num_sms();  // stream-K shares the tail over ALL SMs
-  cudaError_t e = launch_kernel(kern, dim3(grid), dim3(ewg ? kGemmThreadsEwg : kGemmThreads), smem, st, 1, ta, tb, p);
-  if (e != cudaSuccess) {
-    set_error("mm_gemm_fwd: launch failed: %s", cudaGetErrorString(e));
-    return 2;
-  }
-  return check_launch("mm_gemm_fwd");
-}
+// Every launch parameter of one GEMM call.  plan_gemm() alone decides them; mm_gemm_plan() reports `s` and
+// mm_gemm_fwd() encodes its tensor maps and launches from them.
+struct GemmLaunch {
+  GemmKParams p;
+  mm_gemm_schedule s;  // tile grid, kernel variant, grid, threads and dynamic shared memory of the launch
+  bool f16;            // fp16 operands, else bf16
+};
 
-template <int EPI>
-static int launch_gemm_wide(const CUtensorMap& ta, const CUtensorMap& tb, const GemmKParams& p, bool f16, cudaStream_t st) {
-  static bool attr_set[2][kMaxDevices] = {};
-  auto kern = f16 ? gemm_wide_kernel<EPI, true> : gemm_wide_kernel<EPI, false>;
-  if (int rc = ensure_smem_attr(kern, kWideSmemBytes, attr_set[f16 ? 1 : 0], "mm_gemm_fwd")) return rc;
-  const int pairs = p.m_tiles * (p.n_tiles / 2);
-  cudaError_t e = launch_kernel(kern, dim3(pairs < num_sms() ? pairs : num_sms()), dim3(kWideThreads), kWideSmemBytes,
-                                st, 1, ta, tb, p);
-  if (e != cudaSuccess) {
-    set_error("mm_gemm_fwd: launch failed: %s", cudaGetErrorString(e));
-    return 2;
-  }
-  return check_launch("mm_gemm_fwd");
-}
-
-}  // namespace mm
-
-using namespace mm;
-
-// The whole host side of a GEMM call: argument checks, tile width, stream-K decision, rasterisation group, tensor maps,
-// launch.  With `plan` set it stops after the decisions (nothing is dereferenced, encoded or launched): mm_gemm_plan()
-// exposes the schedule to the CPU test tier and to tools/gemm_plan.py.
-static int32_t gemm_dispatch(const mm_gemm_args* a, void* stream, mm_gemm_schedule* plan) {
+// Argument checks (all of them before any decision), then the decisions: tile width, rasterisation group, stream-K
+// tail, kernel variant, launch shape.  Nothing is dereferenced: mm_gemm_plan() runs this without a GPU.
+static int plan_gemm(const mm_gemm_args* a, GemmLaunch& L) {
   MM_REQUIRE(a != nullptr, "mm_gemm_fwd: null args");
   MM_REQUIRE(a->M > 0 && a->N > 0 && a->K > 0 && a->batch > 0 && a->batch2 >= 0,
              "mm_gemm_fwd: bad shape M=%d N=%d K=%d batch=%d batch2=%d", a->M, a->N, a->K, a->batch, a->batch2);
@@ -1083,8 +1055,35 @@ static int32_t gemm_dispatch(const mm_gemm_args* a, void* stream, mm_gemm_schedu
   MM_REQUIRE(a->batch == 1 || (a->a_bs % 8 == 0 && a->b_bs % 8 == 0), "mm_gemm_fwd: batch strides must be multiples of 8");
   MM_REQUIRE(batch2 == 1 || (a->a_bs2 % 8 == 0 && a->b_bs2 % 8 == 0), "mm_gemm_fwd: batch2 strides must be multiples of 8");
   MM_REQUIRE(a->epi >= MM_EPI_STD && a->epi <= MM_EPI_ROPE, "mm_gemm_fwd: bad epilogue %d", a->epi);
-
-  GemmKParams p;
+  MM_REQUIRE(a->sumsq_out == nullptr || (a->epi == MM_EPI_STD && !a->c_trans && !a->c_fp32 && a->batch == 1 && batch2 == 1 &&
+                                         a->N % 32 == 0),
+             "mm_gemm_fwd: sumsq_out needs the standard epilogue, 16-bit output, no batching and N %% 32 == 0");
+  MM_REQUIRE(a->rs_sumsq == nullptr || (a->rs_parts > 0 && a->rs_parts % 4 == 0 && !a->c_trans && a->batch == 1 && batch2 == 1 &&
+                                        (reinterpret_cast<uintptr_t>(a->rs_sumsq) & 15) == 0),
+             "mm_gemm_fwd: rs_sumsq needs rs_parts %% 4 == 0, a 16-byte aligned buffer and no batching");
+  MM_REQUIRE(!(a->c_fp16 && a->c_fp32), "mm_gemm_fwd: c_fp16 and c_fp32 are exclusive");
+  MM_REQUIRE((a->a_fp16 != 0) == (a->b_fp16 != 0),
+             "mm_gemm_fwd: A and B must share one 16-bit format (wgmma takes no mixed f16 x bf16 operands)");
+  MM_REQUIRE((!a->bias_rs && !a->bias2 && !a->bias2_rs) || (a->epi == MM_EPI_STD && !a->c_trans),
+             "mm_gemm_fwd: row-scaled bias terms need the standard, non-transposed epilogue");
+  MM_REQUIRE(!a->c_trans || (a->epi == MM_EPI_STD && a->batch == 1 && batch2 == 1),
+             "mm_gemm_fwd: c_trans needs the standard epilogue and no batching");
+  MM_REQUIRE(!a->a_mn_major || (a->b_mn_major && a->epi == MM_EPI_STD && !a->c_trans),
+             "mm_gemm_fwd: MN-major A needs MN-major B and the standard epilogue");
+  MM_REQUIRE(!a->b_mn_major || a->epi == MM_EPI_STD, "mm_gemm_fwd: MN-major B only with the standard epilogue");
+  // 128-bit epilogue accesses: C, bias and residual 16-byte aligned, their strides whole 16-byte units
+  const int esz = a->c_fp32 ? 4 : 2;
+  bool vec = (reinterpret_cast<uintptr_t>(a->C) % 16 == 0) && ((a->ldc * esz) % 16 == 0) &&
+             ((a->c_bs * esz) % 16 == 0) && ((a->c_bs2 * esz) % 16 == 0);
+  if (a->bias) vec = vec && (reinterpret_cast<uintptr_t>(a->bias) % 16 == 0) && (a->bias_bs % 8 == 0);
+  if (a->residual)
+    vec = vec && (reinterpret_cast<uintptr_t>(a->residual) % 16 == 0) && (a->ldr % 8 == 0) && (a->r_bs % 8 == 0) &&
+          (a->r_bs2 % 8 == 0);
+  MM_REQUIRE(a->epi != MM_EPI_ROPE || (a->N % 128 == 0 && a->rope_cos && a->rope_sin && a->rope_T > 0 && vec &&
+                                       a->rope_cols % 128 == 0),
+             "mm_gemm_fwd: RoPE epilogue needs N %% 128 == 0, cos/sin tables and vector-aligned C");
+  MM_REQUIRE(a->epi != MM_EPI_SWIGLU || a->N % 64 == 0, "mm_gemm_fwd: SwiGLU epilogue needs N %% 64 == 0");
+  GemmKParams& p = L.p;
   p.M = a->M; p.N = a->N; p.K = a->K; p.batch = a->batch; p.batch2 = batch2;
   p.num_k = (a->K + kBlockK - 1) / kBlockK;
   p.m_tiles = (a->M + kBlockM - 1) / kBlockM;
@@ -1104,39 +1103,12 @@ static int32_t gemm_dispatch(const mm_gemm_args* a, void* stream, mm_gemm_schedu
   p.bias_rs = a->bias_rs; p.bias2 = reinterpret_cast<const bf16*>(a->bias2); p.bias2_rs = a->bias2_rs;
   p.sumsq_out = a->sumsq_out; p.sumsq_parts = (a->N + 31) / 32;
   p.rs_sumsq = a->rs_sumsq; p.rs_parts = a->rs_parts; p.rs_eps = a->rs_eps;
-  MM_REQUIRE(a->sumsq_out == nullptr || (a->epi == MM_EPI_STD && !a->c_trans && !a->c_fp32 && a->batch == 1 && batch2 == 1 &&
-                                         a->N % 32 == 0),
-             "mm_gemm_fwd: sumsq_out needs the standard epilogue, 16-bit output, no batching and N %% 32 == 0");
-  MM_REQUIRE(a->rs_sumsq == nullptr || (a->rs_parts > 0 && a->rs_parts % 4 == 0 && !a->c_trans && a->batch == 1 && batch2 == 1 &&
-                                        (reinterpret_cast<uintptr_t>(a->rs_sumsq) & 15) == 0),
-             "mm_gemm_fwd: rs_sumsq needs rs_parts %% 4 == 0, a 16-byte aligned buffer and no batching");
-  MM_REQUIRE(!(a->c_fp16 && a->c_fp32), "mm_gemm_fwd: c_fp16 and c_fp32 are exclusive");
-  MM_REQUIRE((a->a_fp16 != 0) == (a->b_fp16 != 0),
-             "mm_gemm_fwd: A and B must share one 16-bit format (wgmma takes no mixed f16 x bf16 operands)");
-  MM_REQUIRE((!a->bias_rs && !a->bias2 && !a->bias2_rs) || (a->epi == MM_EPI_STD && !a->c_trans),
-             "mm_gemm_fwd: row-scaled bias terms need the standard, non-transposed epilogue");
-  MM_REQUIRE(!(a->c_fp16 && a->c_fp32), "mm_gemm_fwd: c_fp16 and c_fp32 are exclusive");
-  MM_REQUIRE(!a->c_trans || (a->epi == MM_EPI_STD && a->batch == 1 && batch2 == 1),
-             "mm_gemm_fwd: c_trans needs the standard epilogue and no batching");
-
-  const int esz = a->c_fp32 ? 4 : 2;
-  bool vec = (reinterpret_cast<uintptr_t>(a->C) % 16 == 0) && ((a->ldc * esz) % 16 == 0) &&
-             ((a->c_bs * esz) % 16 == 0) && ((a->c_bs2 * esz) % 16 == 0);
-  if (a->bias) vec = vec && (reinterpret_cast<uintptr_t>(a->bias) % 16 == 0) && (a->bias_bs % 8 == 0);
-  if (a->residual)
-    vec = vec && (reinterpret_cast<uintptr_t>(a->residual) % 16 == 0) && (a->ldr % 8 == 0) && (a->r_bs % 8 == 0) &&
-          (a->r_bs2 % 8 == 0);
   p.vec_ok = vec ? 1 : 0;
 
-  // ---- tile width: widest BN that still yields enough tiles to occupy the SMs
+  // ---- tile width: widest BN that still yields enough tiles to occupy the SMs (RoPE and SwiGLU epilogues: 128)
   const int sms = num_sms();
   int BN = kMaxBN;
-  if (a->epi == MM_EPI_ROPE) {
-    MM_REQUIRE(a->N % 128 == 0 && a->rope_cos && a->rope_sin && a->rope_T > 0 && vec && a->rope_cols % 128 == 0,
-               "mm_gemm_fwd: RoPE epilogue needs N %% 128 == 0, cos/sin tables and vector-aligned C");
-  } else if (a->epi == MM_EPI_SWIGLU) {
-    MM_REQUIRE(a->N % 64 == 0, "mm_gemm_fwd: SwiGLU epilogue needs N %% 64 == 0");
-  } else {
+  if (a->epi == MM_EPI_STD) {
     // Cost model (cycles per 64-deep k-block of one tile; two warpgroups of m64nBNk16): the tensor cores need 4 BN cycles
     // (2048 dense bf16 FMA per cycle and SM), shared memory must deliver each warpgroup's 8 KiB of A plus the whole B
     // tile (128 BN bytes) at 128 B/cycle -> 128 + 2 BN cycles.  BN = 64 sits on both limits (10 % penalty).  The model
@@ -1165,14 +1137,13 @@ static int32_t gemm_dispatch(const mm_gemm_args* a, void* stream, mm_gemm_schedu
     if (a->b_mn_major && BN < 64) BN = 64;
   }
   p.n_tiles = (a->N + BN - 1) / BN;
-  static const int gm_env = []() { const char* e = getenv("MACAW_B200_GEMM_GROUPM"); return e ? atoi(e) : 0; }();
   const long long tiles = (long long)a->batch * batch2 * p.m_tiles * p.n_tiles;
   // rasterisation: keep one group's A rows (~16 MiB) resident in the 50 MB L2 while its B tiles stream
   {
     const long long unit_bytes = (long long)kBlockM * a->K * 2;
     long long g = ((16LL << 20) + unit_bytes / 2) / unit_bytes;
     g = g < 2 ? 2 : (g > 32 ? 32 : g);
-    p.group_m = gm_env > 0 ? gm_env : static_cast<int>(g);
+    p.group_m = static_cast<int>(g);
   }
   // ---- stream-K tail: only when the last wave is clearly partial and K is long enough to split
   p.sk_tiles = 0; p.sk_first = 0; p.sk_ws = nullptr; p.sk_flags = nullptr;
@@ -1194,75 +1165,102 @@ static int32_t gemm_dispatch(const mm_gemm_args* a, void* stream, mm_gemm_schedu
       p.sk_ws = reinterpret_cast<float*>(reinterpret_cast<char*>(a->sk_workspace) + 8192);
     }
   }
-  MM_REQUIRE(!a->a_mn_major || (a->b_mn_major && a->epi == MM_EPI_STD && !a->c_trans),
-             "mm_gemm_fwd: MN-major A needs MN-major B and the standard epilogue");
-  MM_REQUIRE(!a->b_mn_major || a->epi == MM_EPI_STD, "mm_gemm_fwd: MN-major B only with the standard epilogue");
-  if (plan != nullptr) {
-    plan->block_n = BN;
-    plan->pairs = 0;
-    plan->m_tiles = p.m_tiles;
-    plan->n_tiles = p.n_tiles;
-    plan->k_blocks = p.num_k;
-    plan->units = tiles;
-    plan->workers = sms;
-    plan->grid = static_cast<int>((tiles < sms && p.sk_tiles == 0) ? tiles : sms);
-    plan->waves = static_cast<int>((tiles + sms - 1) / sms);
-    plan->group_m = p.group_m;
-    plan->streamk_tiles = p.sk_tiles;
-    plan->smem_bytes = static_cast<int32_t>(gemm_smem_bytes(BN));
-    plan->vectorised_epilogue = p.vec_ok;
-    return 0;
+  // ---- kernel variant.  A stream-K launch keeps the consumer epilogue: the epilogue warpgroup handles whole tiles only
+  // (the tail's pieces of one or two k-blocks would leave it nothing to overlap).
+  const int overlap = overlap_mode();
+  const bool ewg = overlap >= 1 && p.num_k >= kEwgMinKBlocks && p.sk_tiles == 0;
+  // Mode 2: launches that the epilogue warpgroup would take, whose 128-wide N tiles pair up without a remainder and fill
+  // at least one wave of pairs, walk those tiles two at a time (gemm_wide_kernel): same tiles, same epilogue, same bits.
+  const bool wide = overlap == 2 && ewg && BN == kMaxBN && !a->a_mn_major && !a->b_mn_major && !a->c_trans &&
+                    a->batch == 1 && batch2 == 1 && p.n_tiles % 2 == 0 && tiles / 2 >= sms;
+  L.f16 = a->a_fp16 != 0;
+  mm_gemm_schedule& s = L.s;
+  s.block_n = BN; s.m_tiles = p.m_tiles; s.n_tiles = p.n_tiles; s.k_blocks = p.num_k; s.group_m = p.group_m;
+  s.units = tiles; s.workers = sms; s.waves = static_cast<int>((tiles + sms - 1) / sms);
+  s.streamk_tiles = p.sk_tiles; s.vectorised_epilogue = p.vec_ok;
+  s.kernel = wide ? MM_GEMM_KERNEL_TILE_PAIRS : ewg ? MM_GEMM_KERNEL_EPILOGUE_WARPGROUP : MM_GEMM_KERNEL_CONSUMER_EPILOGUE;
+  s.threads = wide ? kWideThreads : ewg ? kGemmThreadsEwg : kGemmThreads;
+  s.smem_bytes = static_cast<int32_t>(wide ? kWideSmemBytes : gemm_smem_bytes(gemm_stages(BN), BN * kBlockK * 2, BN));
+  const long long units = wide ? tiles / 2 : tiles;  // what one CTA takes at a time: a tile, or a pair of tiles
+  s.grid = static_cast<int>((units < sms && p.sk_tiles == 0) ? units : sms);  // stream-K shares the tail over ALL SMs
+  MM_REQUIRE(s.kernel == MM_GEMM_KERNEL_CONSUMER_EPILOGUE || p.sk_tiles == 0,
+             "mm_gemm_fwd: only the consumer-epilogue kernel takes a stream-K tail");
+  return 0;
+}
+
+template <auto kern>
+static int launch_gemm(const GemmLaunch& L, const CUtensorMap& ta, const CUtensorMap& tb, cudaStream_t st) {
+  static bool attr_set[kMaxDevices] = {};
+  if (int rc = ensure_smem_attr(kern, L.s.smem_bytes, attr_set, "mm_gemm_fwd")) return rc;
+  cudaError_t e = launch_kernel(kern, dim3(L.s.grid), dim3(L.s.threads), L.s.smem_bytes, st, 1, ta, tb, L.p);
+  if (e != cudaSuccess) {
+    set_error("mm_gemm_fwd: launch failed: %s", cudaGetErrorString(e));
+    return 2;
   }
+  return check_launch("mm_gemm_fwd");
+}
+
+// The kernel instance of a plan: its variant and operand format at the caller's tile width, epilogue and operand layouts.
+// Tile pairs exist for 128-wide tiles of K-major operands only.
+template <int BN, int EPI, bool B_MN = false, bool A_MN = false>
+static int launch_variant(const GemmLaunch& L, const CUtensorMap& ta, const CUtensorMap& tb, cudaStream_t st) {
+  if constexpr (BN == kMaxBN && !B_MN && !A_MN)
+    if (L.s.kernel == MM_GEMM_KERNEL_TILE_PAIRS)
+      return L.f16 ? launch_gemm<&gemm_wide_kernel<EPI, true>>(L, ta, tb, st)
+                   : launch_gemm<&gemm_wide_kernel<EPI, false>>(L, ta, tb, st);
+  if (L.s.kernel == MM_GEMM_KERNEL_EPILOGUE_WARPGROUP)
+    return L.f16 ? launch_gemm<&gemm_bf16_kernel<BN, EPI, B_MN, A_MN, true, true>>(L, ta, tb, st)
+                 : launch_gemm<&gemm_bf16_kernel<BN, EPI, B_MN, A_MN, false, true>>(L, ta, tb, st);
+  return L.f16 ? launch_gemm<&gemm_bf16_kernel<BN, EPI, B_MN, A_MN, true, false>>(L, ta, tb, st)
+               : launch_gemm<&gemm_bf16_kernel<BN, EPI, B_MN, A_MN, false, false>>(L, ta, tb, st);
+}
+
+}  // namespace mm
+
+using namespace mm;
+
+extern "C" int32_t mm_gemm_fwd(const mm_gemm_args* a, void* stream) {
+  GemmLaunch L;
+  if (int rc = plan_gemm(a, L)) return rc;
+  const int BN = L.s.block_n;
+  const int batch2 = L.p.batch2;
   CUtensorMap ta, tb;
   if (a->a_mn_major) {
     if (make_map(&ta, a->A, a->M, a->K, a->batch, batch2, a->lda, a->a_bs, a->a_bs2, 64)) return 1;
   } else if (make_map(&ta, a->A, a->K, a->M, a->batch, batch2, a->lda, a->a_bs, a->a_bs2, kBlockM)) {
     return 1;
   }
-  const uint64_t b_batch = p.b_shared ? 1 : a->batch;
-  const uint64_t b_batch2 = p.b2_shared ? 1 : batch2;
+  const uint64_t b_batch = L.p.b_shared ? 1 : a->batch;
+  const uint64_t b_batch2 = L.p.b2_shared ? 1 : batch2;
   if (!a->b_mn_major) {
     if (make_map(&tb, a->B, a->K, a->N, b_batch, b_batch2, a->ldb, a->b_bs, a->b_bs2, BN)) return 1;
   } else {
     if (make_map(&tb, a->B, a->N, a->K, b_batch, b_batch2, a->ldb, a->b_bs, a->b_bs2, 64)) return 1;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  const bool f16 = a->a_fp16 != 0;
-  // A stream-K launch keeps the consumer epilogue: the epilogue warpgroup handles whole tiles only (the tail's pieces of
-  // one or two k-blocks would leave it nothing to overlap).
-  const bool ewg = overlap_mode() >= 1 && p.num_k >= kEwgMinKBlocks && p.sk_tiles == 0;
-  // Mode 2: launches that the epilogue warpgroup would take, whose 128-wide N tiles pair up without a remainder and fill
-  // at least one wave of pairs, walk those tiles two at a time (gemm_wide_kernel).  The plan above is unchanged: same
-  // tiles, same epilogue, same bits.
-  if (overlap_mode() == 2 && ewg && BN == kMaxBN && !a->a_mn_major && !a->b_mn_major && !a->c_trans && a->batch == 1 &&
-      batch2 == 1 && p.n_tiles % 2 == 0 && tiles / 2 >= sms) {
-    if (a->epi == MM_EPI_ROPE) return launch_gemm_wide<MM_EPI_ROPE>(ta, tb, p, f16, st);
-    if (a->epi == MM_EPI_SWIGLU) return launch_gemm_wide<MM_EPI_SWIGLU>(ta, tb, p, f16, st);
-    return launch_gemm_wide<MM_EPI_STD>(ta, tb, p, f16, st);
-  }
-
-#define MM_LAUNCH(BN_, EPI_, MN_) return launch_gemm<BN_, EPI_, MN_>(ta, tb, p, f16, ewg, st)
-  if (a->epi == MM_EPI_ROPE) MM_LAUNCH(128, MM_EPI_ROPE, false);
-  if (a->epi == MM_EPI_SWIGLU) MM_LAUNCH(128, MM_EPI_SWIGLU, false);
+#define MM_LAUNCH(...) return launch_variant<__VA_ARGS__>(L, ta, tb, st)
+  if (a->epi == MM_EPI_ROPE) MM_LAUNCH(128, MM_EPI_ROPE);
+  if (a->epi == MM_EPI_SWIGLU) MM_LAUNCH(128, MM_EPI_SWIGLU);
   if (a->a_mn_major) {
-    if (BN == 128) return launch_gemm<128, MM_EPI_STD, true, true>(ta, tb, p, f16, ewg, st);
-    return launch_gemm<64, MM_EPI_STD, true, true>(ta, tb, p, f16, ewg, st);
+    if (BN == 128) MM_LAUNCH(128, MM_EPI_STD, true, true);
+    MM_LAUNCH(64, MM_EPI_STD, true, true);
   }
   if (a->b_mn_major) {
     if (BN == 128) MM_LAUNCH(128, MM_EPI_STD, true);
     MM_LAUNCH(64, MM_EPI_STD, true);
   }
-  if (BN == 128) MM_LAUNCH(128, MM_EPI_STD, false);
-  if (BN == 64) MM_LAUNCH(64, MM_EPI_STD, false);
-  MM_LAUNCH(32, MM_EPI_STD, false);
+  if (BN == 128) MM_LAUNCH(128, MM_EPI_STD);
+  if (BN == 64) MM_LAUNCH(64, MM_EPI_STD);
+  MM_LAUNCH(32, MM_EPI_STD);
 #undef MM_LAUNCH
 }
 
-extern "C" int32_t mm_gemm_fwd(const mm_gemm_args* a, void* stream) { return gemm_dispatch(a, stream, nullptr); }
-
 extern "C" int32_t mm_gemm_plan(const mm_gemm_args* a, mm_gemm_schedule* plan) {
   MM_REQUIRE(plan != nullptr, "mm_gemm_plan: null plan");
-  return gemm_dispatch(a, nullptr, plan);
+  GemmLaunch L;
+  if (int rc = plan_gemm(a, L)) return rc;
+  *plan = L.s;
+  return 0;
 }
 
 extern "C" int32_t mm_gemm_streamk_mode(int32_t mode) {

@@ -15,6 +15,7 @@ from ._lib import AlignArgs, AttnArgs, GemmArgs
 
 ACT_NONE, ACT_GELU, ACT_QUICK_GELU, ACT_SILU = 0, 1, 2, 3
 EPI_STD, EPI_SWIGLU, EPI_ROPE = 0, 1, 2
+GEMM_CONSUMER_EPILOGUE, GEMM_EPILOGUE_WARPGROUP, GEMM_TILE_PAIRS = 0, 1, 2  # gemm_plan()["kernel"]: MM_GEMM_KERNEL_*
 
 _BF16 = torch.bfloat16
 _F16 = torch.float16

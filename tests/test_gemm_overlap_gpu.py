@@ -4,8 +4,8 @@ Mode 1 (a dedicated epilogue warpgroup runs a tile's epilogue while the consumer
 loop) keeps the MMA k-order and the per-element epilogue arithmetic of mode 0, so its outputs must equal mode 0's exactly
 (torch.equal), for every epilogue, at the benchmark's batch-32 shapes, at ragged / odd-tile shapes and for the training
 step's MN-major operands, in both activation formats, over repeated launches and a CUDA-graph replay.  Each case also
-checks, from the launched kernel's name, that mode 1 really ran the epilogue warpgroup; launches below 32 k-blocks or
-with a stream-K tail keep the consumer epilogue in every mode."""
+checks, from the launched kernel's name, that mode 1 really ran the epilogue warpgroup and that mm_gemm_plan predicted
+the kernel that ran; launches below 32 k-blocks or with a stream-K tail keep the consumer epilogue in every mode."""
 import re
 
 import pytest
@@ -92,20 +92,44 @@ def _case(kind, M, N, K, dt, seed=0):
     raise ValueError(kind)
 
 
-def _ewg_flags(fn):
-    """The EWG template argument (the last one) of every GEMM kernel `fn` launches, from the profiler's kernel names."""
+def _launched(fn):
+    """The variant (ops.GEMM_*, as in gemm_plan()["kernel"]) of every GEMM kernel `fn` launches, from the profiler's
+    kernel names: gemm_wide_kernel, or gemm_bf16_kernel with the EWG template argument (the last one) false / true."""
     from torch.profiler import ProfilerActivity, profile
 
+    ops = _ops()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         fn()
         torch.cuda.synchronize()
-    flags = []
+    variants = set()
     for ev in prof.events():
+        if "gemm_wide_kernel<" in ev.name:
+            variants.add(ops.GEMM_TILE_PAIRS)
         m = re.search(r"gemm_bf16_kernel<([^>]*)>", ev.name)
         if m:
-            flags.append(m.group(1).split(",")[-1].strip())
-    assert flags, "no GEMM kernel launched"
-    return set(flags)
+            ewg = m.group(1).split(",")[-1].strip() == "true"
+            variants.add(ops.GEMM_EPILOGUE_WARPGROUP if ewg else ops.GEMM_CONSUMER_EPILOGUE)
+    assert variants, "no GEMM kernel launched"
+    return variants
+
+
+def _planned(kind, M, N, K, dt, streamk=False):
+    """The variant ops.gemm_plan predicts, under the current modes, for the GEMM call of _case(kind, M, N, K, dt)."""
+    ops = _ops()
+    kw = dict(M=M, N=N, K=K, fp16=dt == torch.float16, streamk=streamk)
+    if kind == "rope_rms":
+        kw.update(epi=ops.EPI_ROPE)
+    elif kind == "swiglu_rms":
+        kw.update(epi=ops.EPI_SWIGLU)
+    elif kind == "plain_fp32":
+        kw.update(c_fp32=True)
+    elif kind == "thin":  # linear_thin swaps the operands
+        kw.update(M=N, N=M, c_trans=True)
+    elif kind == "dx":
+        kw.update(b_mn_major=True)
+    elif kind == "dw":  # gemm_dw: dW (N x K) = dy^T x over the M rows
+        kw.update(M=N, N=K, K=M, a_mn_major=True, b_mn_major=True)
+    return ops.gemm_plan(**kw)["kernel"]
 
 
 # (kind, M, N, K): the benchmark's batch-32 GEMMs, then odd M-tile counts, ragged edges and the training step's
@@ -139,12 +163,12 @@ def test_overlap_modes_bit_identical(kind, M, N, K, dt):
     for a, b in zip(got, want):
         assert torch.equal(a, b)
     assert all(torch.isfinite(t.float()).all() for t in want)
-    lib = _lib()
+    ops, lib = _ops(), _lib()
     prev = lib.mm_gemm_overlap_mode(0)
     try:
-        assert _ewg_flags(fn) == {"false"}
-        lib.mm_gemm_overlap_mode(1)
-        assert _ewg_flags(fn) == {"true"}  # the case really runs the epilogue warpgroup
+        assert _launched(fn) == {_planned(kind, M, N, K, dt)} == {ops.GEMM_CONSUMER_EPILOGUE}
+        lib.mm_gemm_overlap_mode(1)  # the case really runs the epilogue warpgroup, as planned
+        assert _launched(fn) == {_planned(kind, M, N, K, dt)} == {ops.GEMM_EPILOGUE_WARPGROUP}
     finally:
         lib.mm_gemm_overlap_mode(prev)
 
@@ -162,7 +186,7 @@ def test_short_k_and_streamk_keep_consumer_epilogue(kind, M, N, K, streamk):
     try:
         if streamk:
             assert ops.gemm_plan(M=M, N=N, K=K, fp16=True, streamk=True)["streamk_tiles"] > 0
-        assert _ewg_flags(fn) == {"false"}
+        assert _launched(fn) == {_planned(kind, M, N, K, torch.float16, streamk)} == {ops.GEMM_CONSUMER_EPILOGUE}
     finally:
         ops.STREAMK = None
         lib.mm_gemm_overlap_mode(prev)

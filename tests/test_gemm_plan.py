@@ -1,6 +1,6 @@
-"""CPU tier: the host side of mm_gemm_fwd (tile width from the cost model, rasterisation group, stream-K tail, argument
-checks) through mm_gemm_plan — the same dispatcher run without a launch.  No GPU involved: the library assumes the 132
-SMs of an H100 SXM when no device is visible.  The decisions asserted here are the ones DESIGN.md §3 / §6 document."""
+"""CPU tier: the host side of mm_gemm_fwd (tile width from the cost model, rasterisation group, stream-K tail, kernel
+variant and launch shape, argument checks) through mm_gemm_plan — the same dispatcher run without a launch.  No GPU
+involved: the library assumes the 132 SMs of an H100 SXM when no device is visible.  The decisions asserted here are the ones DESIGN.md §3 / §6 document."""
 import ctypes as C
 import random
 
@@ -10,6 +10,8 @@ from macaw_llm_b200 import _lib, ops
 
 E, I, V = 4096, 11008, 32000
 SMS = 132
+CONSUMER, EWG, PAIRS = ops.GEMM_CONSUMER_EPILOGUE, ops.GEMM_EPILOGUE_WARPGROUP, ops.GEMM_TILE_PAIRS
+SMEM_128, SMEM_64, SMEM_PAIRS = 199936, 183552, 216320  # 4 stages of 128 x 128, 6 of 128 x 64, 3 of 128 x 256
 
 
 def plan(**kw):
@@ -21,7 +23,8 @@ def test_llama_gemms_at_batch_32_use_full_width_tiles():
     for N, K, epi in ((3 * E, E, ops.EPI_ROPE), (E, E, ops.EPI_STD), (2 * I, E, ops.EPI_SWIGLU), (E, I, ops.EPI_STD),
                       (V, E, ops.EPI_STD)):
         p = plan(M=M, N=N, K=K, epi=epi, fp16=True, streamk=True)
-        assert (p["block_n"], p["pairs"], p["grid"], p["workers"]) == (128, 0, SMS, SMS), (N, K, p)
+        assert (p["block_n"], p["grid"], p["workers"]) == (128, SMS, SMS), (N, K, p)
+        assert (p["kernel"], p["threads"], p["smem_bytes"]) == (PAIRS, 384, SMEM_PAIRS), (N, K, p)
         assert p["units"] == (M // 128) * ((N + 127) // 128) and p["waves"] == (N + 127) // 128 and p["streamk_tiles"] == 0
         assert p["smem_bytes"] <= 227 * 1024 and p["vectorised_epilogue"] == 1
     # rasterisation group ~ 16 MiB of A rows: 16 M tiles at K = 4096, 6 at K = 11008
@@ -32,9 +35,11 @@ def test_short_k_gemms_stay_single_cta():
     # CLIP / Whisper layers (K = 1024 / 512)
     for M, N, K in ((8224, 3072, 1024), (8224, 4096, 1024), (48000, 1536, 512), (48000, 2048, 512)):
         p = plan(M=M, N=N, K=K, fp16=True)
-        assert p["pairs"] == 0 and p["workers"] == SMS and p["grid"] == SMS and p["block_n"] == 128, p
+        assert p["workers"] == SMS and p["grid"] == SMS and p["block_n"] == 128, p
+        assert (p["kernel"], p["threads"], p["smem_bytes"]) == (CONSUMER, 288, SMEM_128), p  # < 32 k-blocks
     p = plan(M=8224, N=1024, K=4096, fp16=True)  # fc2: 65 x 8 = 520 tiles of 128 x 128 fill 4 waves (528 slots)
     assert (p["block_n"], p["units"], p["waves"]) == (128, 520, 4)
+    assert (p["kernel"], p["grid"]) == (PAIRS, SMS)  # 260 pairs
 
 
 def test_per_gpu_batch_of_the_8_gpu_run():
@@ -42,17 +47,28 @@ def test_per_gpu_batch_of_the_8_gpu_run():
     M = 4 * 528
     qkv = plan(M=M, N=3 * E, K=E, epi=ops.EPI_ROPE, fp16=True, streamk=True)
     assert (qkv["block_n"], qkv["units"], qkv["waves"], qkv["streamk_tiles"]) == (128, 17 * 96, 13, 0)  # 48-tile tail: too small a saving
+    assert (qkv["kernel"], qkv["grid"]) == (PAIRS, SMS)  # 816 pairs
     gu = plan(M=M, N=2 * I, K=E, epi=ops.EPI_SWIGLU, fp16=True, streamk=True)
     assert (gu["units"], gu["waves"], gu["streamk_tiles"], gu["grid"]) == (17 * 172, 23, (17 * 172) % SMS, SMS)
+    assert (gu["kernel"], gu["threads"], gu["smem_bytes"]) == (CONSUMER, 288, SMEM_128)  # the tail takes the consumer epilogue
     o = plan(M=M, N=E, K=E, fp16=True, streamk=True)  # 64-wide tiles: 9 waves of 128 x 64 beat 5 of 128 x 128
     assert (o["block_n"], o["units"], o["waves"]) == (64, 17 * 64, 9)
+    assert (o["kernel"], o["threads"], o["grid"], o["smem_bytes"]) == (EWG, 512, SMS, SMEM_64)
     head = plan(M=M, N=V, K=E, fp16=True, streamk=True)
     assert (head["block_n"], head["units"], head["waves"], head["grid"]) == (128, 17 * 250, 33, SMS)
+    assert (head["streamk_tiles"], head["kernel"]) == (0, PAIRS)
     assert plan(M=M, N=2 * I, K=E, epi=ops.EPI_SWIGLU, fp16=True, streamk=False)["streamk_tiles"] == 0  # opt-in per launch
 
 
 def test_policy_switches():
     lib = _lib.load()
+    for mode, want in ((0, (CONSUMER, 288, SMEM_128)), (1, (EWG, 512, SMEM_128))):
+        prev = lib.mm_gemm_overlap_mode(mode)
+        try:
+            p = plan(M=32 * 528, N=3 * E, K=E, epi=ops.EPI_ROPE, fp16=True, streamk=True)
+            assert (p["kernel"], p["threads"], p["smem_bytes"], p["grid"]) == want + (SMS,), mode
+        finally:
+            lib.mm_gemm_overlap_mode(prev)
     prev = lib.mm_gemm_streamk_mode(0)
     try:
         assert plan(M=4 * 528, N=2 * I, K=E, epi=ops.EPI_SWIGLU, streamk=True)["streamk_tiles"] == 0
@@ -72,9 +88,20 @@ def test_policy_switches():
 def test_thin_decode_gemms_use_narrow_tiles():
     # swapped operands (c_trans): the weight rows fill the 128-row MMA tile, the 8 token rows are the N extent
     p = plan(M=E, N=8, K=E, c_trans=True)
-    assert p["block_n"] == 32 and p["pairs"] == 0 and p["units"] == E // 128 and p["grid"] == E // 128
+    assert p["block_n"] == 32 and p["units"] == E // 128 and p["grid"] == E // 128
+    assert (p["kernel"], p["threads"], p["smem_bytes"]) == (EWG, 512, SMEM_64)  # 8 stages of 128 x 32: as many bytes
     p = plan(M=E, N=8, K=E // 4, batch=4, c_fp32=True)  # split-K of 4 through the batch dimension: 128 units
     assert p["units"] == 4 * (E // 128) and p["grid"] == 128
+    assert (p["kernel"], p["threads"]) == (CONSUMER, 288)  # 16 k-blocks
+
+
+def test_kernel_variant_of_narrow_and_mn_major_launches():
+    p = plan(M=100, N=E, K=E)  # the cost model picks 128 tiles of 128 x 32: less than a wave
+    assert (p["block_n"], p["units"], p["kernel"], p["threads"], p["grid"]) == (32, 128, EWG, 512, 128)
+    dx = plan(M=4 * 528, N=E, K=I, b_mn_major=True)  # training: dx = dy W
+    dw = plan(M=E, N=E, K=4 * 528, a_mn_major=True, b_mn_major=True)  # training: dW = dy^T x, 33 k-blocks
+    for p in (dx, dw):
+        assert (p["kernel"], p["threads"], p["grid"]) == (EWG, 512, SMS), p
 
 
 def test_schedule_invariants_random_shapes():
@@ -94,7 +121,10 @@ def test_schedule_invariants_random_shapes():
         assert p["block_n"] in (32, 64, 128) and (not b_mn or p["block_n"] >= 64)
         assert p["m_tiles"] == (M + 127) // 128 and p["n_tiles"] == (N + p["block_n"] - 1) // p["block_n"]
         assert p["k_blocks"] == (K + 63) // 64
-        assert p["units"] == batch * p["m_tiles"] * p["n_tiles"] and p["pairs"] == 0
+        assert p["units"] == batch * p["m_tiles"] * p["n_tiles"]
+        assert p["threads"] == {CONSUMER: 288, EWG: 512, PAIRS: 384}[p["kernel"]]
+        assert p["kernel"] == CONSUMER or p["streamk_tiles"] == 0
+        assert p["kernel"] != PAIRS or (batch == 1 and not b_mn and p["n_tiles"] % 2 == 0 and p["smem_bytes"] == SMEM_PAIRS)
         assert p["workers"] == SMS
         assert p["waves"] == -(-p["units"] // p["workers"]) and 0 < p["grid"] <= SMS
         assert 0 <= p["streamk_tiles"] < SMS

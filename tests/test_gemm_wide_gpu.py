@@ -4,28 +4,15 @@ of mode 1.
 The wide kernel walks the same tiles with the same k-order and runs the same epilogue code per tile, so every output must
 equal mode 1's exactly (torch.equal): the decoder's and lm_head's GEMMs at the benchmark's 16896 rows, at 17 M tiles and
 at ragged M / N / K, in both activation formats, over repeated launches and a CUDA-graph replay.  Each case checks from
-the profiler's kernel names that mode 2 really ran the wide kernel; launches that do not qualify (odd number of N tiles,
-fewer than 32 k-blocks, a stream-K tail, MN-major operands) must keep the kernel modes 0 / 1 run."""
-import re
-
+the profiler's kernel names that mode 2 really ran the wide kernel, as mm_gemm_plan predicted; launches that do not
+qualify (odd number of N tiles, fewer than 32 k-blocks, a stream-K tail, MN-major operands) must keep the kernel modes
+0 / 1 run."""
 import pytest
 import torch
 
-from tests.test_gemm_overlap_gpu import E, I, M32, T, V, _case, _lib, _ops, run_mode
+from tests.test_gemm_overlap_gpu import E, I, M32, T, V, _case, _launched, _lib, _ops, _planned, run_mode
 
 pytestmark = pytest.mark.gpu
-
-
-def _gemm_kernels(fn):
-    """Names (without template arguments) of the GEMM kernels `fn` launches."""
-    from torch.profiler import ProfilerActivity, profile
-
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    names = {m.group(1) for ev in prof.events() for m in [re.search(r"(gemm_wide_kernel|gemm_bf16_kernel)<", ev.name)] if m}
-    assert names, "no GEMM kernel launched"
-    return names
 
 
 WIDE = [
@@ -51,12 +38,12 @@ def test_wide_bit_identical_to_mode_1(kind, M, N, K, dt):
     for a, b in zip(got, want):
         assert torch.equal(a, b)
     assert all(torch.isfinite(t.float()).all() for t in want)
-    lib = _lib()
+    ops, lib = _ops(), _lib()
     prev = lib.mm_gemm_overlap_mode(2)
     try:
-        assert _gemm_kernels(fn) == {"gemm_wide_kernel"}
+        assert _launched(fn) == {_planned(kind, M, N, K, dt)} == {ops.GEMM_TILE_PAIRS}
         lib.mm_gemm_overlap_mode(1)
-        assert _gemm_kernels(fn) == {"gemm_bf16_kernel"}
+        assert _launched(fn) == {_planned(kind, M, N, K, dt)} == {ops.GEMM_EPILOGUE_WARPGROUP}
     finally:
         lib.mm_gemm_overlap_mode(prev)
 
@@ -76,7 +63,8 @@ def test_unqualified_launches_keep_the_narrow_kernel(kind, M, N, K, streamk):
     try:
         if streamk:
             assert ops.gemm_plan(M=M, N=N, K=K, fp16=True, streamk=True)["streamk_tiles"] > 0
-        assert _gemm_kernels(fn) == {"gemm_bf16_kernel"}
+        launched = _launched(fn)
+        assert launched == {_planned(kind, M, N, K, torch.float16, streamk)} and ops.GEMM_TILE_PAIRS not in launched
         if want is not None:
             for a, b in zip(fn(), want):
                 assert torch.equal(a, b)

@@ -1,8 +1,9 @@
 """CPU tier: the pair walk of the wide GEMM kernel (`pair_coord` and the round-robin loop of `gemm_wide_kernel`,
 csrc/gemm_wgmma.cu), restated in Python.  The wide kernel is a different walk over the tiles mm_gemm_plan reports, not a
-different tiling, so for every qualifying shape:
-  1. the plan still reports the 128-wide tile grid (block_n 128, pairs 0, units = m_tiles * n_tiles);
-  2. the pairs (m_blk, 2 j), (m_blk, 2 j + 1) visited by CTAs 0 .. grid - 1 cover every tile of that grid exactly once;
+different tiling, so for every launch the plan gives the tile-pair kernel:
+  1. the plan still reports the 128-wide tile grid (block_n 128, units = m_tiles * n_tiles);
+  2. the pairs (m_blk, 2 j), (m_blk, 2 j + 1) visited by the plan's CTAs 0 .. grid - 1 cover every tile of that grid
+     exactly once;
   3. the TMA loader's cursor (one lane of a consumer warp, running ahead of the main loop) visits the same (pair, k-block)
      sequence as the consumers of its CTA;
   4. every index product formed on the device fits a signed 32-bit integer.
@@ -15,6 +16,7 @@ from macaw_llm_b200 import ops
 
 SMS = 132
 E, I, V = 4096, 11008, 32000
+PAIRS = ops.GEMM_TILE_PAIRS
 
 
 def pair_coord(idx, m_tiles, n_tiles, group_m):
@@ -29,16 +31,11 @@ def pair_coord(idx, m_tiles, n_tiles, group_m):
     return first_m + rr % gsz, 2 * (rr // gsz)
 
 
-def goes_wide(p, *, k_min=32):
-    """The dispatcher's rule for overlap mode 2 on a K-major, unbatched launch (gemm_dispatch)."""
-    return (p["block_n"] == 128 and p["k_blocks"] >= k_min and p["streamk_tiles"] == 0 and p["n_tiles"] % 2 == 0 and
-            p["units"] // 2 >= p["workers"])
-
-
 def check_walk(p):
     m_tiles, n_tiles, gm = p["m_tiles"], p["n_tiles"], p["group_m"]
     pairs = m_tiles * (n_tiles // 2)
-    grid = min(pairs, p["workers"])
+    grid = p["grid"]
+    assert 0 < grid <= p["workers"]
     seen = [[0] * n_tiles for _ in range(m_tiles)]
     for worker in range(grid):
         consumer, loader = [], []
@@ -68,10 +65,9 @@ def check_walk(p):
 def test_benchmark_shapes(M, N, K, epi):
     p = ops.gemm_plan(M=M, N=N, K=K, epi=epi, fp16=True)
     if M == 4 * 528 and N == E:
-        assert p["block_n"] == 64 and not goes_wide(p)  # o_proj / down at 17 M tiles: the 64-wide plan stays narrow
+        assert p["block_n"] == 64 and p["kernel"] == ops.GEMM_EPILOGUE_WARPGROUP  # o_proj / down at 17 M tiles
         return
-    assert (p["block_n"], p["pairs"]) == (128, 0) and p["units"] == p["m_tiles"] * p["n_tiles"]
-    assert goes_wide(p)
+    assert (p["block_n"], p["kernel"]) == (128, PAIRS) and p["units"] == p["m_tiles"] * p["n_tiles"]
     if M == 32 * 528:
         assert (p["m_tiles"] * (p["n_tiles"] // 2)) % SMS == 0  # whole waves of pairs at the benchmark's batch
     check_walk(p)
@@ -85,15 +81,16 @@ def test_random_qualifying_shapes():
         N = rng.choice([1024, 1536, 3072, 4000, 4096, 12288, 22016, 32000])
         K = rng.choice([2048, 2120, 4096, 11008])
         p = ops.gemm_plan(M=M, N=N, K=K, fp16=rng.random() < 0.5)
-        if not goes_wide(p):
+        if p["kernel"] != PAIRS:
             continue
         n += 1
-        assert p["pairs"] == 0 and p["units"] == p["m_tiles"] * p["n_tiles"]
+        assert p["block_n"] == 128 and p["units"] == p["m_tiles"] * p["n_tiles"]
         check_walk(p)
 
 
 def test_shapes_that_do_not_qualify():
-    assert not goes_wide(ops.gemm_plan(M=16896, N=E + 128, K=E))      # 33 N tiles
-    assert not goes_wide(ops.gemm_plan(M=16896, N=E, K=1024))         # 16 k-blocks
-    assert not goes_wide(ops.gemm_plan(M=100, N=E, K=E))              # less than one wave of pairs
-    assert not goes_wide(ops.gemm_plan(M=31 * 528, N=E, K=E, streamk=True))  # stream-K tail
+    ewg, consumer = ops.GEMM_EPILOGUE_WARPGROUP, ops.GEMM_CONSUMER_EPILOGUE
+    assert ops.gemm_plan(M=16896, N=E + 128, K=E)["kernel"] == ewg                 # 33 N tiles
+    assert ops.gemm_plan(M=16896, N=E, K=1024)["kernel"] == consumer               # 16 k-blocks
+    assert ops.gemm_plan(M=100, N=E, K=E)["kernel"] == ewg                         # less than one wave of pairs
+    assert ops.gemm_plan(M=31 * 528, N=E, K=E, streamk=True)["kernel"] == consumer  # stream-K tail

@@ -140,7 +140,7 @@ def test_adamw_entries_take_lr_dev_and_keep_the_abi5_argument_list():
             assert fake.got == short, name
 
     lib = _lib.load()
-    assert _lib.ABI_VERSION == 7 and lib.mm_abi_version() == 7
+    assert _lib.ABI_VERSION == 8 and lib.mm_abi_version() == 8
     for name in ("mm_adamw", "mm_adamw_host"):
         fn = getattr(lib, name)
         assert isinstance(fn, _lib._NullableBeforeStream) and len(fn.argtypes) == 18, name

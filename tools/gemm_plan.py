@@ -19,9 +19,7 @@ def row(name, M, N, K, **kw):
     pad = 1.0 - M / (p["m_tiles"] * 128.0)
     eff = p["fill"] * (1.0 - pad) if p["streamk_tiles"] == 0 else (1.0 - pad)  # stream-K shares the tail over all CTAs
     flops = 2.0 * M * N * K
-    # overlap mode 2 (the default) walks these K-major, unbatched launches as N-neighbouring tile pairs when:
-    wide = (p["block_n"] == 128 and p["k_blocks"] >= 32 and p["streamk_tiles"] == 0 and p["n_tiles"] % 2 == 0 and
-            p["units"] // 2 >= p["workers"])
+    wide = p["kernel"] == ops.GEMM_TILE_PAIRS  # N-neighbouring tile pairs (overlap mode 2, the default)
     return (f"  {name:22s} M={M:6d} N={N:6d} K={K:6d}  BN={p['block_n']:3d} units={p['units']:5d} "
             f"waves={p['waves']:3d} fill={p['fill']:.3f} pad={pad:.3f} group_m={p['group_m']:2d} streamk_tiles={p['streamk_tiles']:3d} "
             f"-> useful share of the scheduled MMA slots {eff:.3f}{'  [128x256 main loop]' if wide else ''}"), flops, eff
