@@ -487,6 +487,53 @@ int32_t mm_window_gather_add(const void* dwin, int32_t B, int32_t N, int32_t C, 
                              void* dfeats, void* stream);
 int32_t mm_cast_f16_bf16(const void* x, int64_t ldx, void* y, int64_t ldy, int32_t rows, int32_t cols, void* stream);
 
+/* ------------------------------------------------------------------------------------------------ LoRA adapters
+ * Low-rank adapters on a frozen nn.Linear (PEFT's LoraLayer.forward): y = x W^T + s * drop(x) A^T B^T, s = lora_alpha / r,
+ * A (r, K), B (N, r), drop = inverted dropout with the Philox mask of csrc/philox.cuh (stream sid[j], the training step's
+ * device seed; p = 0 or seed null: off).  The mask of input element (m, k) is that of mm_dropout_mask(row m, col k): the
+ * backward pass regenerates it.  One launch serves n (1..MM_LORA_MAX) adapters of the same shapes; in the down and
+ * dx-backward entries they share the input x (q / k / v, gate / up read it once).  Tensors are 16-bit in the activation
+ * format unless marked fp32; rows are contiguous unless a leading dimension is given; 8 <= r <= 64, r % 8 == 0,
+ * K % 8 == 0.  Every reduction is a fixed-order sum (per-CTA partials in `workspace`): results are deterministic.
+ *   mm_lora_down    u[j] (M, r) fp32 = drop_j(x) A_j^T
+ *   mm_lora_up      y[j] (M, N, ld ldy) <- round(rope(y[j] + s u[j] B_j^T)), in place.  With rope_cos / rope_sin (fp32
+ *                   (T, 64) tables, position = row % rope_T) the rotate-half RoPE over 128-wide heads (pairs c, c + 64)
+ *                   is applied in fp32 before the one rounding (N % 128 == 0): the adapted q / k projection.
+ *   mm_lora_bwd_dy  with dy = y[j] (M, N, ld ldy): g[j] (M, r) fp32 = s dy B_j;  dB[j] (N, r) (+)= s dy^T u[j]
+ *   mm_lora_bwd_x   dA[j] (r, K) (+)= g[j]^T drop_j(x);  dx (M, K, ld lddx) <- round(dx + sum_j drop_j(g[j] A_j)), in place
+ * accumulate[j] != 0 adds the gradient of adapter j to dA[j] / dB[j] (fp32 sum, one rounding), else overwrites them.
+ * mm_lora_workspace_bytes: the fp32 workspace `entry` (2 = bwd_dy, 3 = bwd_x; 0 otherwise) needs for these shapes. */
+#define MM_LORA_MAX 3
+typedef struct mm_lora_args {
+  int32_t n, M, K, N, r;
+  float scaling, p_drop;
+  const uint64_t* seed_dev;
+  uint32_t sid[MM_LORA_MAX];
+  const void* x;
+  int64_t ldx;
+  const void* A[MM_LORA_MAX];
+  const void* B[MM_LORA_MAX];
+  float* u[MM_LORA_MAX];
+  void* y[MM_LORA_MAX];
+  int64_t ldy;
+  const float* rope_cos;
+  const float* rope_sin;
+  int32_t rope_T;
+  float* g[MM_LORA_MAX];
+  void* dA[MM_LORA_MAX];
+  void* dB[MM_LORA_MAX];
+  int32_t accumulate[MM_LORA_MAX];
+  void* dx;
+  int64_t lddx;
+  float* workspace;
+  int64_t workspace_bytes;
+} mm_lora_args;
+int32_t mm_lora_down(const mm_lora_args* args, void* stream);
+int32_t mm_lora_up(const mm_lora_args* args, void* stream);
+int32_t mm_lora_bwd_dy(const mm_lora_args* args, void* stream);
+int32_t mm_lora_bwd_x(const mm_lora_args* args, void* stream);
+int64_t mm_lora_workspace_bytes(const mm_lora_args* args, int32_t entry);
+
 /* ------------------------------------------------------------------------------------------------ gradient all-reduce
  * The one collective of the path: the data-parallel gradient all-reduce of the training step (reference: DeepSpeed ZeRO-3
  * reduce-scatter / all-gather, configs/deepspeed_config.json:22-41; north_star: "a single NCCL all-reduce on gradients").

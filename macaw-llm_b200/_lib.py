@@ -77,6 +77,21 @@ class AlignArgs(C.Structure):
     ]
 
 
+LORA_MAX = 3
+
+
+class LoraArgs(C.Structure):
+    """Mirror of `mm_lora_args` (include/macaw_b200.h)."""
+
+    _fields_ = [
+        ("n", c_i32), ("M", c_i32), ("K", c_i32), ("N", c_i32), ("r", c_i32), ("scaling", c_f32), ("p_drop", c_f32),
+        ("seed_dev", c_vp), ("sid", c_u32 * LORA_MAX), ("x", c_vp), ("ldx", c_i64), ("A", c_vp * LORA_MAX),
+        ("B", c_vp * LORA_MAX), ("u", c_vp * LORA_MAX), ("y", c_vp * LORA_MAX), ("ldy", c_i64), ("rope_cos", c_vp),
+        ("rope_sin", c_vp), ("rope_T", c_i32), ("g", c_vp * LORA_MAX), ("dA", c_vp * LORA_MAX), ("dB", c_vp * LORA_MAX),
+        ("accumulate", c_i32 * LORA_MAX), ("dx", c_vp), ("lddx", c_i64), ("workspace", c_vp), ("workspace_bytes", c_i64),
+    ]
+
+
 class LossScaleState(C.Structure):
     """Mirror of `mm_loss_scale_state` (include/macaw_b200.h): 12 four-byte fields."""
 
@@ -163,6 +178,11 @@ SIGNATURES = {
     "mm_nccl_allreduce": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp]),
     "mm_nccl_destroy": (c_i32, []),
     "mm_ce_loss": (c_i32, [c_vp, c_vp, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp]),
+    "mm_lora_down": (c_i32, [C.POINTER(LoraArgs), c_vp]),
+    "mm_lora_up": (c_i32, [C.POINTER(LoraArgs), c_vp]),
+    "mm_lora_bwd_dy": (c_i32, [C.POINTER(LoraArgs), c_vp]),
+    "mm_lora_bwd_x": (c_i32, [C.POINTER(LoraArgs), c_vp]),
+    "mm_lora_workspace_bytes": (c_i64, [C.POINTER(LoraArgs), c_i32]),
 }
 
 # Nullable pointers added to an entry after it first shipped, just before its final `stream` argument: a Python call may

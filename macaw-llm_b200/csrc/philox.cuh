@@ -15,6 +15,10 @@ namespace mm {
 // Stream id of the token sampler (mm_sample_rows).  The dropout sites use 1..4 (Engine.DROPOUT_SID); the sampler's
 // words come from counter = (step, row, SID_SAMPLE, 0) and never coincide with a dropout mask's.
 constexpr uint32_t SID_SAMPLE = 16u;
+// Stream ids of the LoRA adapters' input dropout (mm_lora_*; lora.lora_sid mirrors them): the lm_head adapter uses
+// SID_LORA_LM_HEAD, the adapter on target t (0..6: q, k, v, o, gate, up, down) of decoder layer l uses SID_LORA0 + 8 l + t.
+constexpr uint32_t SID_LORA_LM_HEAD = 24u;
+constexpr uint32_t SID_LORA0 = 32u;
 
 __host__ __device__ inline void philox_round(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
   const uint64_t p0 = static_cast<uint64_t>(0xD2511F53u) * c[0];

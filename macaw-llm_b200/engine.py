@@ -17,7 +17,7 @@ from typing import Dict, Optional, Tuple
 
 import torch
 
-from . import ops
+from . import lora, ops
 
 BF16 = torch.bfloat16
 
@@ -542,15 +542,25 @@ class Engine:
         k = f"llm.l{i}."
         sa, mlp = l.self_attn, l.mlp
         g1, g2 = l.input_layernorm.weight, l.post_attention_layernorm.weight
-        wqkv = self.derived(k + "wqkv", [sa.q_proj.weight, sa.k_proj.weight, sa.v_proj.weight, g1],
-                            lambda: (torch.cat([sa.q_proj.weight, sa.k_proj.weight, sa.v_proj.weight], 0).detach().float()
+        # LoRA adapters are folded in: lora.merged_weight is W + s B A in fp32 for an adapted projection (W otherwise)
+        wqkv = self.derived(k + "wqkv", lora.weight_params(sa.q_proj) + lora.weight_params(sa.k_proj)
+                            + lora.weight_params(sa.v_proj) + [g1],
+                            lambda: (torch.cat([lora.merged_weight(sa.q_proj), lora.merged_weight(sa.k_proj),
+                                                lora.merged_weight(sa.v_proj)], 0)
                                      * g1.detach().float()[None, :]).to(ADT()).contiguous())
-        wgu = self.derived(k + "wgu", [mlp.gate_proj.weight, mlp.up_proj.weight, g2],
+        wgu = self.derived(k + "wgu", lora.weight_params(mlp.gate_proj) + lora.weight_params(mlp.up_proj) + [g2],
                            lambda: torch.stack(
-                               [(mlp.gate_proj.weight.detach().float() * g2.detach().float()[None, :]).to(ADT()).view(I // 32, 32, E),
-                                (mlp.up_proj.weight.detach().float() * g2.detach().float()[None, :]).to(ADT()).view(I // 32, 32, E)], 1)
+                               [(lora.merged_weight(mlp.gate_proj) * g2.detach().float()[None, :]).to(ADT()).view(I // 32, 32, E),
+                                (lora.merged_weight(mlp.up_proj) * g2.detach().float()[None, :]).to(ADT()).view(I // 32, 32, E)], 1)
                            .reshape(2 * I, E).contiguous())
-        return wqkv, wgu, self.w(sa.o_proj.weight, k + "wo"), self.w(mlp.down_proj.weight, k + "wd")
+        return wqkv, wgu, self._linear_weight(sa.o_proj, k + "wo"), self._linear_weight(mlp.down_proj, k + "wd")
+
+    def _linear_weight(self, lin, key: str) -> torch.Tensor:
+        """The weight of a linear layer in the activation format, its LoRA adapter merged in when it carries one."""
+        if not lora.is_adapted(lin):
+            return self.w(lin.weight, key)
+        return self.derived("lora:" + key, lora.weight_params(lin),
+                            lambda: lora.merged_weight(lin).to(ADT()).contiguous())
 
     def _llama_dims(self):
         cfg = self.m.llm.config
@@ -652,8 +662,8 @@ class Engine:
         """final RMSNorm (as the row scale of the GEMM) + lm_head on the rows of x (reference modeling.py:508, 597)."""
         llm = self.m.llm
         gn = llm.model.norm.weight
-        wl = self.derived("llm.lm_head_g", [llm.lm_head.weight, gn],
-                          lambda: (llm.lm_head.weight.detach().float() * gn.detach().float()[None, :]).to(ADT()).contiguous())
+        wl = self.derived("llm.lm_head_g", lora.weight_params(llm.lm_head) + [gn],
+                          lambda: (lora.merged_weight(llm.lm_head) * gn.detach().float()[None, :]).to(ADT()).contiguous())
         ops.TAG = "lm_head"
         ss, self._last_ss = getattr(self, "_last_ss", None), None
         if rows is None and x.shape[0] > 64 and ss is not None and ss.shape[0] == x.shape[0]:

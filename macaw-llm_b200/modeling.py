@@ -398,6 +398,31 @@ class MM_LLMs(PreTrainedModel):
             self.__dict__["_train_step"] = TrainStep(self)
         return self.__dict__["_train_step"]
 
+    # ---- LoRA adapters on the decoder (lora.py; reference run_clm_llms.py:498-508, run_clm_llms_inference.py:88-94) ----
+    def add_lora(self, config):
+        """`get_peft_model(model.llm, config)`: adapters on the targeted decoder projections, base decoder frozen."""
+        from . import lora
+
+        return lora.add_lora(self, config)
+
+    def save_lora(self, directory: str) -> None:
+        """PEFT's adapter layout: adapter_config.json + adapter_model.bin."""
+        from . import lora
+
+        lora.save_lora(self, directory)
+
+    def load_lora(self, directory: str) -> None:
+        """`PeftModel.from_pretrained(model.llm, directory)` (adds the adapters first when the model has none)."""
+        from . import lora
+
+        lora.load_lora(self, directory)
+
+    def merge_lora(self) -> None:
+        """`merge_and_unload()`: the adapters are folded into the base weights and removed."""
+        from . import lora
+
+        lora.merge_lora(self)
+
     def prepare_inputs_for_generation(self, inputs):
         return self._engine.prepare_inputs(inputs)
 

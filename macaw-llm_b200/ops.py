@@ -924,3 +924,112 @@ def window_gather_add(dwin: torch.Tensor, B: int, N: int, C: int, Lq: int, kk: i
     _check(_lib.load().mm_window_gather_add(dwin.data_ptr(), B, N, C, Lq, kk, ss, out.data_ptr(), _stream()),
            "mm_window_gather_add")
     return out
+
+
+# ---------------------------------------------------------------------------------------------------- LoRA adapters
+def _lora_args(M: int, K: int, N: int, r: int, n: int, scaling: float = 1.0, dropout=None) -> "_lib.LoraArgs":
+    """mm_lora_args for n adapters; dropout = None | (p, seed_dev int64 (1,), [stream id per adapter])."""
+    assert 1 <= n <= _lib.LORA_MAX
+    a = _lib.LoraArgs()
+    a.n, a.M, a.K, a.N, a.r, a.scaling = n, M, K, N, r, float(scaling)
+    if dropout is not None and float(dropout[0]) > 0.0:
+        p, seed, sids = dropout
+        _cuda(seed, torch.int64, "seed")
+        assert seed.numel() == 1 and len(sids) == n
+        a.p_drop, a.seed_dev = float(p), seed.data_ptr()
+        for j, s in enumerate(sids):
+            a.sid[j] = int(s)
+    return a
+
+
+def _lora_weights(As, Bs):
+    for A in As:
+        _cuda(A, ACT(), "lora_A")
+        assert A.is_contiguous()
+    for Bw in Bs:
+        _cuda(Bw, ACT(), "lora_B")
+        assert Bw.is_contiguous()
+
+
+def lora_down(x: torch.Tensor, As, dropout=None):
+    """u_j (M, r) fp32 = drop_j(x) A_j^T for adapters sharing the input x (M, K) (mm_lora_down); As: lora_A weights (r, K)."""
+    _cuda(x, ACT(), "x")
+    _lora_weights(As, ())
+    assert x.dim() == 2 and x.stride(1) == 1
+    M, K = x.shape
+    r = As[0].shape[0]
+    assert all(A.shape == (r, K) for A in As)
+    a = _lora_args(M, K, 1, r, len(As), dropout=dropout)
+    a.x, a.ldx = x.data_ptr(), x.stride(0)
+    us = [torch.empty((M, r), device=x.device, dtype=torch.float32) for _ in As]
+    for j, (A, u) in enumerate(zip(As, us)):
+        a.A[j], a.u[j] = A.data_ptr(), u.data_ptr()
+    _check(_lib.load().mm_lora_down(C.byref(a), _stream()), "mm_lora_down")
+    return us
+
+
+def lora_up(ys, us, Bs, scaling: float, rope=None) -> None:
+    """In place: y_j <- round(rope(y_j + scaling u_j B_j^T)) (mm_lora_up); ys (M, N) 16-bit views with unit inner stride and
+    one row stride, us (M, r) fp32, Bs lora_B weights (N, r); rope = (cos, sin, T) applies RoPE over 128-wide heads."""
+    _lora_weights((), Bs)
+    M, N = ys[0].shape
+    r = Bs[0].shape[1]
+    for y, u, Bw in zip(ys, us, Bs):
+        _cuda(y, ACT(), "y"); _cuda(u, torch.float32, "u")
+        assert y.shape == (M, N) and y.stride(1) == 1 and y.stride(0) == ys[0].stride(0)
+        assert u.shape == (M, r) and u.is_contiguous() and Bw.shape == (N, r)
+    a = _lora_args(M, 8, N, r, len(ys), scaling)
+    a.ldy = ys[0].stride(0)
+    for j, (y, u, Bw) in enumerate(zip(ys, us, Bs)):
+        a.y[j], a.u[j], a.B[j] = y.data_ptr(), u.data_ptr(), Bw.data_ptr()
+    if rope is not None:
+        cos, sin, T = rope
+        a.rope_cos, a.rope_sin, a.rope_T = cos.data_ptr(), sin.data_ptr(), int(T)
+    _check(_lib.load().mm_lora_up(C.byref(a), _stream()), "mm_lora_up")
+
+
+def lora_bwd_dy(dys, us, Bs, dBs, scaling: float, accumulate):
+    """g_j (M, r) fp32 = scaling dy_j B_j and dB_j (+)= scaling dy_j^T u_j (mm_lora_bwd_dy) -> [g_j]; dBs: gradient views
+    (N, r) in the activation format, accumulate[j]: add into dB_j instead of overwriting it."""
+    _lora_weights((), Bs)
+    M, N = dys[0].shape
+    r = Bs[0].shape[1]
+    for dy, u, Bw, dB in zip(dys, us, Bs, dBs):
+        _cuda(dy, ACT(), "dy"); _cuda(u, torch.float32, "u"); _cuda(dB, ACT(), "dB")
+        assert dy.shape == (M, N) and dy.stride(1) == 1 and dy.stride(0) == dys[0].stride(0)
+        assert u.shape == (M, r) and u.is_contiguous() and Bw.shape == (N, r) and dB.shape == (N, r) and dB.is_contiguous()
+    a = _lora_args(M, 8, N, r, len(dys), scaling)
+    a.ldy = dys[0].stride(0)
+    gs = [torch.empty((M, r), device=dys[0].device, dtype=torch.float32) for _ in dys]
+    for j, (dy, u, Bw, dB, g) in enumerate(zip(dys, us, Bs, dBs, gs)):
+        a.y[j], a.u[j], a.B[j], a.dB[j], a.g[j] = dy.data_ptr(), u.data_ptr(), Bw.data_ptr(), dB.data_ptr(), g.data_ptr()
+        a.accumulate[j] = int(bool(accumulate[j]))
+    lib = _lib.load()
+    ws = torch.empty(((int(lib.mm_lora_workspace_bytes(C.byref(a), 2)) + 15) // 16 * 4,), device=dys[0].device,
+                     dtype=torch.float32)
+    a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel() * 4
+    _check(lib.mm_lora_bwd_dy(C.byref(a), _stream()), "mm_lora_bwd_dy")
+    return gs
+
+
+def lora_bwd_x(x: torch.Tensor, gs, As, dAs, dx: torch.Tensor, accumulate, dropout=None) -> None:
+    """dA_j (+)= g_j^T drop_j(x) and, in place, dx <- round(dx + sum_j drop_j(g_j A_j)) for adapters sharing the input x
+    (mm_lora_bwd_x); dropout as in lora_down (the same masks)."""
+    _cuda(x, ACT(), "x"); _cuda(dx, ACT(), "dx")
+    _lora_weights(As, ())
+    M, K = x.shape
+    r = As[0].shape[0]
+    assert x.stride(1) == 1 and dx.shape == (M, K) and dx.stride(1) == 1
+    for g, A, dA in zip(gs, As, dAs):
+        _cuda(g, torch.float32, "g"); _cuda(dA, ACT(), "dA")
+        assert g.shape == (M, r) and g.is_contiguous() and A.shape == (r, K) and dA.shape == (r, K) and dA.is_contiguous()
+    a = _lora_args(M, K, 1, r, len(As), dropout=dropout)
+    a.x, a.ldx, a.dx, a.lddx = x.data_ptr(), x.stride(0), dx.data_ptr(), dx.stride(0)
+    for j, (g, A, dA) in enumerate(zip(gs, As, dAs)):
+        a.g[j], a.A[j], a.dA[j] = g.data_ptr(), A.data_ptr(), dA.data_ptr()
+        a.accumulate[j] = int(bool(accumulate[j]))
+    lib = _lib.load()
+    ws = torch.empty(((int(lib.mm_lora_workspace_bytes(C.byref(a), 3)) + 15) // 16 * 4,), device=x.device,
+                     dtype=torch.float32)
+    a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel() * 4
+    _check(lib.mm_lora_bwd_x(C.byref(a), _stream()), "mm_lora_bwd_x")
