@@ -579,6 +579,62 @@ int32_t mm_image_preprocess(const mm_image_args* args, void* stream);
 int32_t mm_log_mel(const float* pcm, int32_t n_samples, const float* basisT, const float* mel, float* logspec,
                    void* max_scratch, void* out, int32_t out_fp32, void* stream);
 
+/* mm_jpeg_decode: a batch of sequential Huffman JPEG files (8-bit, grayscale or YCbCr with luma sampling 1x1 / 2x1 / 2x2
+ * and chroma 1x1, one scan) decoded bit-exactly as libjpeg-turbo does with its defaults (ISLOW IDCT, fancy upsampling,
+ * fixed-point YCbCr -> RGB), in three kernels:
+ *   1. entropy decode, one thread per entropy-coded segment (a restart interval, or the whole scan): int16 coefficients,
+ *      natural order, per component in block order (coef + coef_off[c], block (by, bx) at (by * bw[c] + bx) * 64);
+ *   2. dequantise + ISLOW IDCT: uint8 component planes padded to whole blocks (planes + plane_off[c], row stride bw[c] * 8);
+ *   3. fancy upsampling + YCbCr -> RGB: HWC uint8 at out + out_off, row stride out_ld bytes.
+ * The host parses the markers and packs every file's scan bytes into `data` and the descriptors below into device memory.
+ * Whatever the bytes, the kernels read inside their segment and write inside their image's buffers; an inconsistency sets
+ * bits of status[image] (zeroed by the call): 1 invalid Huffman code, 2 coefficient run past 63, 4 segment ends early,
+ * 8 bytes left over after a segment's last MCU, 16 bad byte stuffing, 32 descriptor out of range.  max_blocks / max_pixels:
+ * the batch's largest component block count and largest width * height (launch geometry). */
+typedef struct mm_jpeg_image {
+  int32_t width, height;
+  int32_t n_comp;             /* 1 or 3 */
+  int32_t hmax, vmax;         /* luma sampling factors; chroma is 1 x 1 (1 x 1 for grayscale) */
+  int32_t mcus_x, mcus_y;
+  int32_t seg0, n_seg;        /* segments[seg0 .. seg0 + n_seg) */
+  int32_t bw[3], bh[3];       /* blocks per row / column of each component (whole MCUs) */
+  int32_t huff_dc[3], huff_ac[3]; /* indices into huff[] */
+  int32_t quant[3];           /* indices into quant[] */
+  int64_t coef_off[3];        /* int16 elements */
+  int64_t plane_off[3];       /* bytes */
+  int64_t out_off, out_ld;    /* bytes */
+} mm_jpeg_image;
+typedef struct mm_jpeg_segment {
+  int64_t offset;             /* bytes into data, markers excluded */
+  int32_t n_bytes;
+  int32_t image;
+  int32_t mcu0, n_mcu;
+} mm_jpeg_segment;
+typedef struct mm_jpeg_huff {   /* libjpeg's derived table (jdhuff.c jpeg_make_d_derived_tbl) */
+  int32_t maxcode[18];          /* largest code of each length, -1 if none; [17] = 0xFFFFF */
+  int32_t valoffset[18];        /* huffval index = code + valoffset[length] */
+  uint16_t look[256];           /* 8-bit lookahead: (length << 8) | symbol, 0 = code longer than 8 bits */
+  uint8_t huffval[256];
+} mm_jpeg_huff;
+typedef struct mm_jpeg_args {
+  int32_t n_images, n_segments, n_huff, n_quant;
+  const uint8_t* data;
+  int64_t data_bytes;
+  const mm_jpeg_image* images;
+  const mm_jpeg_segment* segments;
+  const mm_jpeg_huff* huff;
+  const uint16_t* quant;      /* [n_quant][64], natural order */
+  int16_t* coef;
+  int64_t coef_elems;
+  uint8_t* planes;
+  int64_t plane_bytes;
+  uint8_t* out;
+  int64_t out_bytes;
+  int32_t* status;            /* [n_images] */
+  int32_t max_blocks, max_pixels;
+} mm_jpeg_args;
+int32_t mm_jpeg_decode(const mm_jpeg_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

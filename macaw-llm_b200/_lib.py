@@ -110,6 +110,40 @@ class ImageArgs(C.Structure):
     ]
 
 
+class JpegImage(C.Structure):
+    """Mirror of `mm_jpeg_image` (include/macaw_b200.h)."""
+
+    _fields_ = [
+        ("width", c_i32), ("height", c_i32), ("n_comp", c_i32), ("hmax", c_i32), ("vmax", c_i32),
+        ("mcus_x", c_i32), ("mcus_y", c_i32), ("seg0", c_i32), ("n_seg", c_i32),
+        ("bw", c_i32 * 3), ("bh", c_i32 * 3), ("huff_dc", c_i32 * 3), ("huff_ac", c_i32 * 3), ("quant", c_i32 * 3),
+        ("coef_off", c_i64 * 3), ("plane_off", c_i64 * 3), ("out_off", c_i64), ("out_ld", c_i64),
+    ]
+
+
+class JpegSegment(C.Structure):
+    """Mirror of `mm_jpeg_segment` (include/macaw_b200.h)."""
+
+    _fields_ = [("offset", c_i64), ("n_bytes", c_i32), ("image", c_i32), ("mcu0", c_i32), ("n_mcu", c_i32)]
+
+
+class JpegHuff(C.Structure):
+    """Mirror of `mm_jpeg_huff` (include/macaw_b200.h)."""
+
+    _fields_ = [("maxcode", c_i32 * 18), ("valoffset", c_i32 * 18), ("look", C.c_uint16 * 256), ("huffval", C.c_uint8 * 256)]
+
+
+class JpegArgs(C.Structure):
+    """Mirror of `mm_jpeg_args` (include/macaw_b200.h)."""
+
+    _fields_ = [
+        ("n_images", c_i32), ("n_segments", c_i32), ("n_huff", c_i32), ("n_quant", c_i32),
+        ("data", c_vp), ("data_bytes", c_i64), ("images", c_vp), ("segments", c_vp), ("huff", c_vp), ("quant", c_vp),
+        ("coef", c_vp), ("coef_elems", c_i64), ("planes", c_vp), ("plane_bytes", c_i64), ("out", c_vp),
+        ("out_bytes", c_i64), ("status", c_vp), ("max_blocks", c_i32), ("max_pixels", c_i32),
+    ]
+
+
 # name -> (restype, argtypes).  Every symbol declared in include/macaw_b200.h must appear here
 # (tests/test_abi.py cross-checks the header against this table and against the built library).
 SIGNATURES = {
@@ -183,6 +217,7 @@ SIGNATURES = {
     "mm_lora_bwd_dy": (c_i32, [C.POINTER(LoraArgs), c_vp]),
     "mm_lora_bwd_x": (c_i32, [C.POINTER(LoraArgs), c_vp]),
     "mm_lora_workspace_bytes": (c_i64, [C.POINTER(LoraArgs), c_i32]),
+    "mm_jpeg_decode": (c_i32, [C.POINTER(JpegArgs), c_vp]),
 }
 
 # Nullable pointers added to an entry after it first shipped, just before its final `stream` argument: a Python call may

@@ -12,8 +12,8 @@
 //                           80-bin mel projection, log10(clamp 1e-10), max(x, max - 8), (x + 4) / 4.  The 400-point DFT is
 //                           evaluated directly in fp32 (402 x 400 real basis with the window folded in).
 //
-// JPEG / audio container decoding stays on the host (PIL / ffmpeg in the reference): the kernels take decoded 8-bit RGB
-// pixels and PCM samples.  All kernels are HBM / L2 bound integer or fp32 CUDA-core work (no tensor-core reshaping).
+// The kernels take decoded 8-bit RGB pixels and PCM samples: JPEG files are decoded on the device by jpeg.cu, audio
+// containers on the host (ffmpeg in the reference).  All kernels are HBM / L2 bound integer or fp32 CUDA-core work (no tensor-core reshaping).
 #include "common.cuh"
 #include "ptx.cuh"
 #include "../../include/macaw_b200.h"

@@ -10,7 +10,11 @@
   (llm_trainer.py:338-345)                                    STFT / mel / log / clamp pipeline (30 s -> 80 x 3000)
   .half(), .to(device)  (:366-379)                            outputs are produced on the device in the model dtype
 
-JPEG / audio-container DECODING stays on the host (PIL / ffmpeg in the reference): this module takes decoded arrays.
+JPEG files (images and pre-extracted video frames, `'{}{}.mp4_{}.jpg'` in the reference) are decoded on the device too,
+bit-exactly as Pillow decodes them (jpeg.py, csrc/jpeg.cu): `image()`, `images()`, `videos()` and `get_self_inputs()` take
+JPEG bytes or file paths next to decoded arrays, and every JPEG of one call goes through one batched decode.  Files the
+device decoder refuses (progressive, CMYK, ...) raise; decode those on the host and pass the array.  Audio-container
+decoding stays on the host (ffmpeg in the reference): this module takes decoded PCM.
 The coefficient tables of the resize are built here with Pillow's exact double-precision arithmetic (Resample.c:
 precompute_coeffs + normalize_coeffs_8bpc) and cached per source size; the windowed DFT basis and the mel filter bank
 (librosa's Slaney filters, as shipped in whisper/assets/mel_filters.npz) are built once per device.
@@ -24,7 +28,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 import torch
 
-from . import _lib, ops, wire
+from . import _lib, jpeg, ops, wire
 
 CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)   # llm_trainer.py:157
 CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
@@ -114,9 +118,27 @@ class DeviceInputPipeline:
             self._tables[(h, w)] = t
         return t
 
-    def image(self, rgb: torch.Tensor, out: Optional[torch.Tensor] = None, want_u8: bool = False, fp32: bool = False):
-        """One decoded image: uint8 (H, W, 3) RGB (host or device) -> (3, size, size) in the pipeline dtype (fp32 when asked).
-        Returns (tensor, uint8 HWC resized+cropped image | None)."""
+    def decode_jpegs(self, items: Sequence) -> List[torch.Tensor]:
+        """JPEG files (`bytes`, or `str` / `os.PathLike` paths) -> uint8 (H, W, 3) RGB device tensors, decoded in one batch
+        on the device, bit-exact with `np.asarray(Image.open(f))` (grayscale files come back with the plane replicated).
+        Raises NotImplementedError for a JPEG variant the decoder does not support, ValueError for a corrupt file."""
+        return jpeg.decode(items, self.dev)
+
+    def _decode_items(self, images: Sequence, videos: Sequence) -> Tuple[list, list]:
+        """images / videos with every JPEG item replaced by its decoded array, all of them in one batched decode."""
+        items = [r for r in images if jpeg.is_item(r)] + [f for fs in videos if fs is not None for f in fs if jpeg.is_item(f)]
+        if not items:
+            return list(images), list(videos)
+        it = iter(self.decode_jpegs(items))
+        images = [next(it) if jpeg.is_item(r) else r for r in images]
+        videos = [fs if fs is None else [next(it) if jpeg.is_item(f) else f for f in fs] for fs in videos]
+        return images, videos
+
+    def image(self, rgb, out: Optional[torch.Tensor] = None, want_u8: bool = False, fp32: bool = False):
+        """One image: uint8 (H, W, 3) RGB (host or device), or a JPEG file (bytes / path, decoded on the device) ->
+        (3, size, size) in the pipeline dtype (fp32 when asked).  Returns (tensor, uint8 HWC resized+cropped image | None)."""
+        if jpeg.is_item(rgb):
+            rgb = self.decode_jpegs([rgb])[0]
         if rgb.dtype != torch.uint8 or rgb.dim() != 3 or rgb.shape[2] != 3:
             raise ValueError("image(): expected a uint8 (H, W, 3) RGB array (decode / convert('RGB') on the host first)")
         src = rgb.to(self.dev, non_blocking=True).contiguous()
@@ -140,7 +162,8 @@ class DeviceInputPipeline:
         return out, u8
 
     def images(self, rgbs: Sequence[Optional[torch.Tensor]]) -> torch.Tensor:
-        """A batch of decoded images (None = absent -> zeros, llm_trainer.py:352) -> (B, 3, size, size)."""
+        """A batch of images, decoded arrays or JPEG files (None = absent -> zeros, llm_trainer.py:352) -> (B, 3, size, size)."""
+        rgbs, _ = self._decode_items(rgbs, [])
         out = torch.zeros((len(rgbs), 3, self.size, self.size), device=self.dev, dtype=self.dtype)
         for i, r in enumerate(rgbs):
             if r is not None:
@@ -148,7 +171,9 @@ class DeviceInputPipeline:
         return out
 
     def videos(self, frames: Sequence[Optional[Sequence[torch.Tensor]]]) -> torch.Tensor:
-        """Per sample a list of n_frames decoded frames (None = absent -> zeros, llm_trainer.py:315) -> (B, F, 3, S, S)."""
+        """Per sample a list of n_frames frames, decoded arrays or JPEG files (None = absent -> zeros, llm_trainer.py:315)
+        -> (B, F, 3, S, S)."""
+        _, frames = self._decode_items([], frames)
         out = torch.zeros((len(frames), self.n_frames, 3, self.size, self.size), device=self.dev, dtype=self.dtype)
         for i, fs in enumerate(frames):
             if fs is None:
@@ -202,9 +227,11 @@ class DeviceInputPipeline:
     # ---- the reference's get_self_inputs
     def get_self_inputs(self, batch: Dict[str, torch.Tensor], images: Sequence[Optional[torch.Tensor]],
                         audios: Sequence[Optional[torch.Tensor]], videos: Sequence[Optional[Sequence[torch.Tensor]]]) -> dict:
-        """llm_trainer.py:306-381 with decoded media instead of file names: `batch` carries input_ids / attention_mask /
+        """llm_trainer.py:306-381 with media instead of file names: images and video frames as decoded arrays or JPEG files
+        (all JPEGs of the call decoded in one batch), audio as decoded PCM; `batch` carries input_ids / attention_mask /
         labels (wire.collate); returns {'inputs': {...}} exactly like the reference."""
         dev = self.dev
+        images, videos = self._decode_items(images, videos)
         d = {
             "videos": self.videos(videos), "audios": self.audios(audios), "images": self.images(images),
             "input_ids": batch["input_ids"].to(dev), "attention_mask": batch["attention_mask"].to(dev),

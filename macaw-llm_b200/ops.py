@@ -1033,3 +1033,23 @@ def lora_bwd_x(x: torch.Tensor, gs, As, dAs, dx: torch.Tensor, accumulate, dropo
                      dtype=torch.float32)
     a.workspace, a.workspace_bytes = ws.data_ptr(), ws.numel() * 4
     _check(lib.mm_lora_bwd_x(C.byref(a), _stream()), "mm_lora_bwd_x")
+
+
+# ---------------------------------------------------------------------------------------------------- JPEG decode
+def jpeg_decode(data: torch.Tensor, desc: torch.Tensor, layout: dict):
+    """mm_jpeg_decode over a packed batch (jpeg.pack): `data` the scan bytes and `desc` the descriptor bytes, both uint8
+    device tensors.  Allocates the coefficient, plane and output buffers; returns (out uint8, status int32 per image)
+    without synchronising."""
+    _cuda(data, torch.uint8, "data"); _cuda(desc, torch.uint8, "desc")
+    dev = data.device
+    coef = torch.empty(layout["coef"], dtype=torch.int16, device=dev)
+    planes = torch.empty(layout["planes"], dtype=torch.uint8, device=dev)
+    out = torch.empty(layout["out"], dtype=torch.uint8, device=dev)
+    status = torch.empty(layout["n_images"], dtype=torch.int32, device=dev)
+    base, off = desc.data_ptr(), layout["off"]
+    a = _lib.JpegArgs(layout["n_images"], layout["n_segments"], layout["n_huff"], layout["n_quant"], data.data_ptr(),
+                      layout["data_bytes"], base + off["images"], base + off["segments"], base + off["huff"],
+                      base + off["quant"], coef.data_ptr(), coef.numel(), planes.data_ptr(), planes.numel(),
+                      out.data_ptr(), out.numel(), status.data_ptr(), layout["max_blocks"], layout["max_pixels"])
+    _check(_lib.load().mm_jpeg_decode(C.byref(a), _stream()), "mm_jpeg_decode")
+    return out, status

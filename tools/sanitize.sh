@@ -29,3 +29,8 @@ timeout 900 compute-sanitizer --tool racecheck --error-exitcode 9 --print-limit 
 echo "racecheck (GEMM overlap modes) rc=$?"
 timeout 900 compute-sanitizer --tool synccheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_gemm_overlap_gpu.py -q -x -m gpu -k "bit_identical and (bias_gelu-300x1000x2120 or row_scale_alpha-2112x4096x4096)" --timeout 850 --timeout-method=thread 2>&1 | tail -8
 echo "synccheck (GEMM overlap modes) rc=$?"
+# device JPEG decoder: the entropy kernel's bounds checks on corrupt scans, the IDCT's shared-memory column / row passes
+timeout 600 compute-sanitizer --tool memcheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_jpeg_gpu.py -q -x -m gpu --timeout 550 --timeout-method=thread 2>&1 | tail -8
+echo "memcheck (JPEG decode) rc=$?"
+timeout 600 compute-sanitizer --tool racecheck --error-exitcode 9 --print-limit 5 python -m pytest tests/test_jpeg_gpu.py -q -x -m gpu -k "bit_exactly or corrupt" --timeout 550 --timeout-method=thread 2>&1 | tail -8
+echo "racecheck (JPEG decode) rc=$?"
