@@ -534,6 +534,45 @@ int32_t mm_lora_bwd_dy(const mm_lora_args* args, void* stream);
 int32_t mm_lora_bwd_x(const mm_lora_args* args, void* stream);
 int64_t mm_lora_workspace_bytes(const mm_lora_args* args, int32_t entry);
 
+/* ------------------------------------------------------------------------------------------------ int8 decoder weights
+ * Weight-only int8 with one fp32 scale per output row (csrc/quant.cu).
+ *
+ * mm_quantize_rows_int8: w (rows, K) with row stride ldw, format w_format (0 bf16, 1 fp16, 2 fp32) ->
+ *   s[n] = fp32(max_k |w[n][k]|) / 127 (IEEE division), q[n][k] = clamp(rint(fp32(w[n][k]) / s[n]), -127, 127) (round half
+ *   to even), q = 0 where s = 0.  q is (rows, K) contiguous, s is [rows].
+ *
+ * An mm_w8_matrix describes a FUSED weight matrix (N, K) whose rows live in up to MM_W8_MAX_SRC separate int8 matrices: the
+ * device table `chunks` [N / 32][2] names, for fused rows 32c .. 32c + 31, the source j and its first row (the decoder's
+ * [q; k; v] concatenation and [32 gate | 32 up] interleave need no copy of the weights).  Source j is q[j] (rows[j], K)
+ * contiguous with scales scale[j] [rows[j]] (rows[j] % 32 == 0).  gain: [K] 16-bit (activation format) RMSNorm gain, or null.  N % 64 == 0,
+ * K % 16 == 0.
+ *
+ * mm_dequant_rows: out (N, K, row stride ldo, activation format) = round16(fp32(fp32(q s) g)) (without gain:
+ *   round16(fp32(q s))) — the fused 16-bit weight the prefill GEMMs read.
+ * mm_gemm_w8_thin: the split-K partial sums of a decode GEMM for the mm_thin_fused tail,
+ *   part[s][n][m] (row stride ldp >= M) = s_n * sum_{k in slice s} q[n][k] x~[m][k],   x~ = round16(x[m][k] g[k]),
+ *   x (M <= 64, K) 16-bit with row stride ldx (ldx % 8 == 0).  Slice s covers the 128-column stages
+ *   [s ns / splits, (s + 1) ns / splits), ns = ceil(K / 128); 1 <= splits <= ns.  xs_work: 16-bit scratch of
+ *   M * 128 * ns elements.  When the x~ rows of the longest slice (M rounded up to 8 / 16 / 32 / 64, 256 bytes per row per
+ *   stage) fit MM_W8_XS_BYTES they are staged in shared memory once per CTA; otherwise x~ is first written to xs_work and
+ *   streamed through the pipeline with the weights (one more launch).
+ * A chunk-table entry that does not name 32 rows of a present source contributes zero rows. */
+#define MM_W8_MAX_SRC 3
+#define MM_W8_XS_BYTES 49152
+typedef struct mm_w8_matrix {
+  const int8_t* q[MM_W8_MAX_SRC];
+  const float* scale[MM_W8_MAX_SRC];
+  int32_t rows[MM_W8_MAX_SRC];
+  const int32_t* chunks;
+  int32_t N, K;
+  const void* gain;
+} mm_w8_matrix;
+int32_t mm_quantize_rows_int8(const void* w, int64_t ldw, int32_t w_format, int32_t rows, int32_t K, int8_t* q, float* scale,
+                              void* stream);
+int32_t mm_dequant_rows(const mm_w8_matrix* w, void* out, int64_t ldo, void* stream);
+int32_t mm_gemm_w8_thin(const mm_w8_matrix* w, const void* x, int64_t ldx, int32_t M, float* part, int32_t splits,
+                        int32_t ldp, void* xs_work, void* stream);
+
 /* ------------------------------------------------------------------------------------------------ gradient all-reduce
  * The one collective of the path: the data-parallel gradient all-reduce of the training step (reference: DeepSpeed ZeRO-3
  * reduce-scatter / all-gather, configs/deepspeed_config.json:22-41; north_star: "a single NCCL all-reduce on gradients").

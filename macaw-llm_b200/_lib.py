@@ -92,6 +92,17 @@ class LoraArgs(C.Structure):
     ]
 
 
+W8_MAX_SRC = 3
+W8_XS_BYTES = 49152  # MM_W8_XS_BYTES
+
+
+class W8Matrix(C.Structure):
+    """Mirror of `mm_w8_matrix` (include/macaw_b200.h)."""
+
+    _fields_ = [("q", c_vp * W8_MAX_SRC), ("scale", c_vp * W8_MAX_SRC), ("rows", c_i32 * W8_MAX_SRC), ("chunks", c_vp), ("N", c_i32), ("K", c_i32),
+                ("gain", c_vp)]
+
+
 class LossScaleState(C.Structure):
     """Mirror of `mm_loss_scale_state` (include/macaw_b200.h): 12 four-byte fields."""
 
@@ -218,6 +229,9 @@ SIGNATURES = {
     "mm_lora_bwd_x": (c_i32, [C.POINTER(LoraArgs), c_vp]),
     "mm_lora_workspace_bytes": (c_i64, [C.POINTER(LoraArgs), c_i32]),
     "mm_jpeg_decode": (c_i32, [C.POINTER(JpegArgs), c_vp]),
+    "mm_quantize_rows_int8": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp]),
+    "mm_dequant_rows": (c_i32, [C.POINTER(W8Matrix), c_vp, c_i64, c_vp]),
+    "mm_gemm_w8_thin": (c_i32, [C.POINTER(W8Matrix), c_vp, c_i64, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp]),
 }
 
 # Nullable pointers added to an entry after it first shipped, just before its final `stream` argument: a Python call may

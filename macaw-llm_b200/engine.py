@@ -17,7 +17,7 @@ from typing import Dict, Optional, Tuple
 
 import torch
 
-from . import lora, ops
+from . import lora, ops, quant
 
 BF16 = torch.bfloat16
 
@@ -56,6 +56,12 @@ class Engine:
     @staticmethod
     def _stamp(*params) -> tuple:
         return tuple((p.data_ptr(), p._version, p.dtype) for p in params)
+
+    def drop_derived(self) -> None:
+        """Forget every derived weight, captured forward graph and decode state (the parameters were replaced)."""
+        self._cache.clear()
+        self._graphs.clear()
+        self._decode.clear()
 
     def derived(self, key: str, params, fn):
         st = self._stamp(*params)
@@ -555,6 +561,17 @@ class Engine:
                            .reshape(2 * I, E).contiguous())
         return wqkv, wgu, self._linear_weight(sa.o_proj, k + "wo"), self._linear_weight(mlp.down_proj, k + "wd")
 
+    def _w8_layer(self, i: int, l):
+        """The int8 weights of a quantized decoder layer as fused matrices: [q; k; v] and [gate | up] with their RMSNorm
+        gains (applied to the activation rows by the decode GEMM, folded into the rows by the dequantization), o, down."""
+        sa, mlp = l.self_attn, l.mlp
+        g1 = self.w(l.input_layernorm.weight, f"llm.l{i}.g1")
+        g2 = self.w(l.post_attention_layernorm.weight, f"llm.l{i}.g2")
+        src = lambda *ms: ([m.weight for m in ms], [m.weight_scale for m in ms])
+        return (ops.W8Matrix(*src(sa.q_proj, sa.k_proj, sa.v_proj), gain=g1),
+                ops.W8Matrix(*src(mlp.gate_proj, mlp.up_proj), interleave=True, gain=g2),
+                ops.W8Matrix(*src(sa.o_proj)), ops.W8Matrix(*src(mlp.down_proj)))
+
     def _linear_weight(self, lin, key: str) -> torch.Tensor:
         """The weight of a linear layer in the activation format, its LoRA adapter merged in when it carries one."""
         if not lora.is_adapted(lin):
@@ -620,12 +637,26 @@ class Engine:
         decode = cache is not None and T == 1 and B <= 64
         ss_attn = torch.empty((M, E // 32), device=dev, dtype=torch.float32)
         ss_mlp = torch.empty((M, E // 32), device=dev, dtype=torch.float32)
+        # int8 decoder (quant.py): decode steps run the int8 GEMM ahead of the same tails; everything else dequantizes one
+        # layer at a time into one scratch buffer and runs the 16-bit GEMMs below unchanged
+        w8 = quant.is_quantized(self.m)
+        thin = ops.linear_w8_thin_fused if w8 else ops.linear_thin_fused
+        if w8 and not decode:
+            scratch = torch.empty((3 * E + 2 * I + E) * E + E * I, device=dev, dtype=ADT())
+            views, off = [], 0
+            for n, k in ((3 * E, E), (2 * I, E), (E, E), (E, I)):
+                views.append(scratch[off:off + n * k].view(n, k))
+                off += n * k
         for i, l in enumerate(self.m.llm.model.layers):
-            wqkv, wgu, wo, wd = self._llama_weights(i, l, E, I)
+            if w8:
+                mats = self._w8_layer(i, l)
+                wqkv, wgu, wo, wd = mats if decode else [ops.dequant_rows(m, out=v) for m, v in zip(mats, views)]
+            else:
+                wqkv, wgu, wo, wd = self._llama_weights(i, l, E, I)
             rs_kw = dict(row_scale=ops.rms_rstd(x, eps)) if i == 0 else dict(rms_from=(ss_mlp, eps))
             if decode:
-                qkv = ops.linear_thin_fused(x, wqkv, ops.THIN_QKV, rope=(rope[0], rope[1], rope[4] if len(rope) > 4 else None),
-                                            cache=cache[i], t0=pos0, t0_dev=pos_dev[0:1] if dyn else None, **rs_kw)
+                qkv = thin(x, wqkv, ops.THIN_QKV, rope=(rope[0], rope[1], rope[4] if len(rope) > 4 else None),
+                           cache=cache[i], t0=pos0, t0_dev=pos_dev[0:1] if dyn else None, **rs_kw)
             else:
                 qkv = ops.linear(x, wqkv, epi=ops.EPI_ROPE, rope=rope, **rs_kw)
                 if cache is not None:
@@ -641,9 +672,9 @@ class Engine:
                 kv = cache[i][:, : pos0 + T].unflatten(-1, (H, hd))  # (B, Tk, 2, H, hd) view of the cache
                 a = ops.attention(q5[:, :, 0], kv[:, :, 0], kv[:, :, 1], scale=scale, causal=False, key_mask=kmask)
             if decode:
-                ops.linear_thin_fused(a.view(B * T, E), wo, ops.THIN_RES, residual=x, out=x, sumsq_out=ss_attn)
-                g = ops.linear_thin_fused(x, wgu, ops.THIN_SWIGLU, rms_from=(ss_attn, eps))
-                ops.linear_thin_fused(g, wd, ops.THIN_RES, residual=x, out=x, sumsq_out=ss_mlp)
+                thin(a.view(B * T, E), wo, ops.THIN_RES, residual=x, out=x, sumsq_out=ss_attn)
+                g = thin(x, wgu, ops.THIN_SWIGLU, rms_from=(ss_attn, eps))
+                thin(g, wd, ops.THIN_RES, residual=x, out=x, sumsq_out=ss_mlp)
             else:
                 ops.linear(a.view(B * T, E), wo, residual=x, out=x, sumsq_out=ss_attn)
                 g = ops.linear(x, wgu, epi=ops.EPI_SWIGLU, rms_from=(ss_attn, eps))

@@ -380,8 +380,12 @@ class MM_LLMs(PreTrainedModel):
         `loss.backward()`): the loss is produced by the kernel-library training step (training.py) and carries a grad_fn
         whose backward runs the hand-written backward pass.  Logits are not returned in this mode (they are consumed in
         place by the cross-entropy backward)."""
+        from .quant import is_quantized
         from .training import TrainStep
 
+        if is_quantized(self):
+            raise RuntimeError("macaw_b200: the decoder is int8-quantized (quantize_llm_int8) and cannot be trained; call "
+                               "model.eval() / torch.no_grad() for inference")
         if "_train_step" not in self.__dict__:
             self.__dict__["_train_step"] = TrainStep(self)
         if inputs.get("labels") is None:
@@ -422,6 +426,14 @@ class MM_LLMs(PreTrainedModel):
         from . import lora
 
         lora.merge_lora(self)
+
+    # ---- int8 decoder weights (quant.py) ----
+    def quantize_llm_int8(self) -> None:
+        """Weight-only int8 for the seven projections of every decoder layer (per-row fp32 scales), in place; inference
+        only.  lm_head, embed_tokens, the norms, the alignment blocks and the encoders stay 16-bit."""
+        from . import quant
+
+        quant.quantize_llm_int8(self)
 
     def prepare_inputs_for_generation(self, inputs):
         return self._engine.prepare_inputs(inputs)

@@ -247,6 +247,15 @@ def linear_thin_fused(x: torch.Tensor, w: torch.Tensor, mode: int, *, row_scale:
     # fixed split-K factor; the tail kernel adds the partial sums up
     gemm_raw(M=N, N=M, K=Kc, batch=S, A=w.data_ptr(), lda=w.stride(0), a_bs=Kc, B=x.data_ptr(), ldb=x.stride(0), b_bs=Kc,
              Cout=part.data_ptr(), ldc=Mp, c_bs=N * Mp, c_fp32=True, streamk=sk)
+    return _thin_tail(part, M, K, mode, row_scale=row_scale, rms_from=rms_from, residual=residual, out=out,
+                      sumsq_out=sumsq_out, rope=rope, cache=cache, t0=t0, t0_dev=t0_dev)
+
+
+def _thin_tail(part: torch.Tensor, M: int, K: int, mode: int, *, row_scale=None, rms_from=None, residual=None, out=None,
+               sumsq_out=None, rope=None, cache=None, t0: int = 0, t0_dev=None) -> torch.Tensor:
+    """mm_thin_fused over the split-K partial sums part (S, N, Mp) of a thin GEMM with M rows and K columns."""
+    S, N, Mp = part.shape
+    dev = part.device
     n_out = N // 2 if mode == THIN_SWIGLU else N
     if out is None:
         out = torch.empty((M, n_out), device=dev, dtype=ACT())
@@ -275,6 +284,113 @@ def linear_thin_fused(x: torch.Tensor, w: torch.Tensor, mode: int, *, row_scale:
         a.cache, a.Tmax, a.t0, a.t0_dev = cache.data_ptr(), cache.shape[1], int(t0), _ptr(t0_dev)
     _check(_lib.load().mm_thin_fused(C.byref(a), _stream()), "mm_thin_fused")
     return out
+
+
+# ---------------------------------------------------------------------------------------------------- int8 weights
+_W8_FORMAT = {torch.bfloat16: 0, torch.float16: 1, torch.float32: 2}  # mm_quantize_rows_int8's w_format
+
+
+def quantize_rows_int8(w: torch.Tensor):
+    """Per-row int8 quantization of a (rows, K) bf16 / fp16 / fp32 weight (mm_quantize_rows_int8) -> (q int8 (rows, K),
+    scale fp32 (rows,)):  s = fp32(max |w|) / 127,  q = clamp(rint(w / s), -127, 127),  q = 0 where s = 0."""
+    if not isinstance(w, torch.Tensor) or w.dim() != 2 or w.dtype not in _W8_FORMAT or w.stride(1) != 1:
+        raise TypeError("macaw_b200: quantize_rows_int8 takes a 2-D bf16 / fp16 / fp32 tensor with unit column stride")
+    _cuda(w, None, "w")
+    rows, K = w.shape
+    q = torch.empty((rows, K), device=w.device, dtype=torch.int8)
+    s = torch.empty((rows,), device=w.device, dtype=torch.float32)
+    _check(_lib.load().mm_quantize_rows_int8(w.data_ptr(), w.stride(0), _W8_FORMAT[w.dtype], rows, K, q.data_ptr(),
+                                             s.data_ptr(), _stream()), "mm_quantize_rows_int8")
+    return q, s
+
+
+def w8_chunk_map(rows, interleave: bool = False) -> torch.Tensor:
+    """The (source, first source row) of every 32-row chunk of a fused weight matrix, int32 (N / 32, 2) on the CPU.
+    interleave=False: the sources' rows one after another (torch.cat, the [q; k; v] weight); True: two sources of equal
+    height in alternating 32-row groups (fused row 64j + r is row 32j + r of source 0, row 64j + 32 + r of source 1: the
+    [gate | up] weight)."""
+    rows = [int(r) for r in rows]
+    if any(r <= 0 or r % 32 for r in rows):
+        raise ValueError(f"macaw_b200: fused sources need a positive multiple of 32 rows, got {rows}")
+    if interleave:
+        if len(rows) != 2 or rows[0] != rows[1]:
+            raise ValueError(f"macaw_b200: an interleaved fused matrix has two sources of equal height, got {rows}")
+        c = torch.arange(2 * rows[0] // 32)
+        return torch.stack([c % 2, 32 * (c // 2)], 1).to(torch.int32)
+    return torch.cat([torch.stack([torch.full((r // 32,), j), 32 * torch.arange(r // 32)], 1)
+                      for j, r in enumerate(rows)]).to(torch.int32)
+
+
+_W8_CHUNKS = {}  # device copies of the chunk maps, by (rows, interleave, device)
+
+
+class W8Matrix:
+    """A fused int8 weight (N, K) over up to three per-row-quantized sources (mm_w8_matrix), the sources' rows arranged
+    as `w8_chunk_map(rows, interleave)` says; `gain` (K,) 16-bit: the RMSNorm gain folded into the product, or None."""
+
+    def __init__(self, qs, scales, interleave: bool = False, gain: Optional[torch.Tensor] = None):
+        qs, scales = list(qs), list(scales)
+        if not 1 <= len(qs) <= _lib.W8_MAX_SRC or len(scales) != len(qs):
+            raise ValueError(f"macaw_b200: a fused int8 weight has 1..{_lib.W8_MAX_SRC} sources, each with its scales")
+        K = qs[0].shape[1]
+        for q, s in zip(qs, scales):
+            if q.dtype != torch.int8 or q.dim() != 2 or not q.is_contiguous() or q.shape[1] != K:
+                raise TypeError("macaw_b200: int8 sources must be contiguous (rows, K) int8 tensors with one K")
+            if s.dtype != torch.float32 or tuple(s.shape) != (q.shape[0],) or not s.is_contiguous():
+                raise TypeError("macaw_b200: each source needs a contiguous fp32 scale per row")
+        chunks = w8_chunk_map([q.shape[0] for q in qs], interleave)
+        N = 32 * chunks.shape[0]
+        if N % 64 or K % 16:
+            raise ValueError(f"macaw_b200: int8 weights need N % 64 == 0 and K % 16 == 0, got N={N}, K={K}")
+        if gain is not None and (gain.dtype != ACT() or tuple(gain.shape) != (K,) or not gain.is_contiguous()):
+            raise TypeError(f"macaw_b200: the gain must be a contiguous ({K},) {ACT()} tensor")
+        for i, t in enumerate(qs + scales + ([gain] if gain is not None else [])):
+            _cuda(t, None, f"int8 weight operand {i}")
+        dev = qs[0].device
+        key = (tuple(q.shape[0] for q in qs), bool(interleave), str(dev))
+        dchunks = _W8_CHUNKS.get(key)
+        if dchunks is None:
+            dchunks = _W8_CHUNKS[key] = chunks.to(dev)
+        self.N, self.K = N, K
+        self._keep = (qs, scales, dchunks, gain)
+        self.args = _lib.W8Matrix()
+        for j, (q, s) in enumerate(zip(qs, scales)):
+            self.args.q[j], self.args.scale[j], self.args.rows[j] = q.data_ptr(), s.data_ptr(), q.shape[0]
+        self.args.chunks, self.args.N, self.args.K, self.args.gain = dchunks.data_ptr(), N, K, _ptr(gain)
+
+
+def dequant_rows(w: W8Matrix, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The fused 16-bit weight (N, K) in the activation format: round16(fp32(fp32(q s) g)) (mm_dequant_rows)."""
+    dev = w._keep[0][0].device
+    if out is None:
+        out = torch.empty((w.N, w.K), device=dev, dtype=ACT())
+    _cuda(out, ACT(), "out")
+    assert out.shape == (w.N, w.K) and out.stride(1) == 1
+    _check(_lib.load().mm_dequant_rows(C.byref(w.args), out.data_ptr(), out.stride(0), _stream()), "mm_dequant_rows")
+    return out
+
+
+def w8_thin_splits(N: int, K: int, n_sms: int) -> int:
+    """K slices of an int8 decode GEMM: at least two, and enough CTAs (64 weight rows each) for two per SM; at most one
+    slice per 128-column stage.  With two slices the x~ of up to 8 activation rows of a 4096-column slice half fits the
+    kernel's staging buffer, so one-token decode steps at small batch need no extra launch."""
+    return min((K + 127) // 128, max(2, -(-2 * n_sms // (N // 64))))
+
+
+def linear_w8_thin_fused(x: torch.Tensor, w: W8Matrix, mode: int, *, splits: Optional[int] = None, **tail) -> torch.Tensor:
+    """`linear_thin_fused` on an int8 fused weight: mm_gemm_w8_thin writes the split-K partial sums
+    s_n * sum_k q[n, k] round16(x[m, k] g[k]) and the same mm_thin_fused tail finishes them (keywords as there)."""
+    _cuda(x, ACT(), "x")
+    M, K = x.shape
+    assert x.stride(1) == 1 and K == w.K and 1 <= M <= 64
+    dev = x.device
+    S = w8_thin_splits(w.N, K, torch.cuda.get_device_properties(dev).multi_processor_count) if splits is None else int(splits)
+    Mp = (M + 3) // 4 * 4
+    part = torch.empty((S, w.N, Mp), device=dev, dtype=torch.float32)
+    xs_work = torch.empty((M, (K + 127) // 128 * 128), device=dev, dtype=ACT())  # x~ when it is streamed
+    _check(_lib.load().mm_gemm_w8_thin(C.byref(w.args), x.data_ptr(), x.stride(0), M, part.data_ptr(), S, Mp,
+                                       xs_work.data_ptr(), _stream()), "mm_gemm_w8_thin")
+    return _thin_tail(part, M, K, mode, **tail)
 
 
 def splitk_reduce(partial: torch.Tensor, bias: Optional[torch.Tensor], out: torch.Tensor) -> torch.Tensor:

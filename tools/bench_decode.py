@@ -4,7 +4,14 @@ Prints prefill ms and ms per decode step / tokens per second.  Not the benchmark
 
 --sample: greedy and sampled decoding (--temperature / --top-k / --top-p / --repetition-penalty, Vicuna's
 generation_config by default) in one process, alternated over three rounds, then mm_sample_rows alone against
-mm_argmax_rows (CUDA events, V = 32007) at 1, 8 and 64 rows.  Runs in fp16 unless --dtype says otherwise."""
+mm_argmax_rows (CUDA events, V = 32007) at 1, 8 and 64 rows.  Runs in fp16 unless --dtype says otherwise.
+
+--int8: the 16-bit model and a twin built from the same seed and quantized (quantize_llm_int8), fp16 unless --dtype says
+otherwise: peak device memory of each (measured with only that model's working set counted), five alternated rounds of
+prefill ms and decode ms/step at B = 1, 8, 64 and two at B = 96, then each decode GEMM with its tail alone (one call per
+layer captured in a CUDA graph and replayed between CUDA events, so no host time is counted and, with the weights of all
+32 layers in turn, nothing is served from L2): the 16-bit linear_thin_fused against the int8 linear_w8_thin_fused at
+M = 1, 8, 64, with the weight bytes each streams per second as a share of 3.35 TB/s."""
 import argparse
 import os
 import subprocess
@@ -60,6 +67,115 @@ def _kernel_us(ops, rows, V, launches, cfg):
     return out
 
 
+HBM_BPS = 3.35e12  # H100 SXM data sheet
+
+
+def _gemm_us(fn, n_layers, replays):
+    """Kernel time of fn(i) (a GEMM + tail on layer i's weights) per call: one call per layer captured in a CUDA graph,
+    the graph replayed `replays` times between CUDA events (no host launch cost in the window)."""
+    for i in range(n_layers):  # warm-up: function attributes, allocator pool
+        fn(i)
+    torch.cuda.synchronize()
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g):
+        for i in range(n_layers):
+            fn(i)
+    g.replay()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(replays):
+        g.replay()
+    e1.record()
+    e1.synchronize()
+    return e0.elapsed_time(e1) / (replays * n_layers) * 1e3
+
+
+def _int8(a, cfg, dtype):
+    from macaw_llm_b200 import ops
+    from macaw_llm_b200.modeling import MM_LLMs
+
+    llama = cfg.llm_config
+    batches = (1, 8, 64)
+    inputs = {}
+    for B in batches:
+        host = bench.synth_inputs(B, a.seq_len, llama.vocab_size, 224, 3000, 1234)
+        host["audios"] = None
+        inputs[B] = {k: (v.cuda() if isinstance(v, torch.Tensor) else v) for k, v in host.items()}
+    print(f"[bench_decode] {_card()}; int8 decoder vs 16-bit, {dtype}, T={a.seq_len + 8}, new={a.new}, B={batches}")
+    # the quantized twin first: its peak is measured alone; the 16-bit model's peak is measured above the twin's residency
+    models = {}
+    qm = MM_LLMs.build_random(cfg, device="cuda", dtype=dtype, seed=0)
+    qm.quantize_llm_int8()
+    for name, m in (("int8", qm), ("16-bit", None)):
+        if m is None:
+            m = MM_LLMs.build_random(cfg, device="cuda", dtype=dtype, seed=0)
+        torch.cuda.synchronize()
+        torch.cuda.empty_cache()
+        torch.cuda.reset_peak_memory_stats()
+        base = 0 if name == "int8" else resident_q
+        for B in batches:  # warm-up: weight caches, KV caches and decode graphs of every batch size
+            m.engine.generate(inputs[B], max_new_tokens=a.new, eos_token_id=-1)
+        torch.cuda.synchronize()
+        peak = torch.cuda.max_memory_allocated() - base
+        if name == "int8":
+            resident_q = torch.cuda.memory_allocated()
+        models[name] = m
+        print(f"[bench_decode] {name:6s} peak memory allocated with B = {batches} warmed up: {peak / 2 ** 30:.2f} GiB")
+    for rnd in range(5):
+        for B in batches:
+            res = {name: _decode_ms(m.engine, inputs[B], a.new) for name, m in models.items()}
+            print(f"[bench_decode] round {rnd} B={B:2d}: " + "; ".join(
+                f"{n} prefill {p:.1f} ms, decode {s:.3f} ms/step" for n, (p, s) in res.items()))
+    # B > 64: no thin decode path; the int8 model dequantizes every layer in every step.  The KV caches of the smaller
+    # batches are dropped first to make room.
+    big = 96
+    host = bench.synth_inputs(big, a.seq_len, llama.vocab_size, 224, 3000, 1234)
+    host["audios"] = None
+    inp_big = {k: (v.cuda() if isinstance(v, torch.Tensor) else v) for k, v in host.items()}
+    for m in models.values():
+        m.engine._decode.clear()
+    torch.cuda.empty_cache()
+    for m in models.values():
+        m.engine.generate(inp_big, max_new_tokens=a.new, eos_token_id=-1)
+    for rnd in range(2):
+        res = {name: _decode_ms(m.engine, inp_big, a.new) for name, m in models.items()}
+        print(f"[bench_decode] round {rnd} B={big}: " + "; ".join(
+            f"{n} prefill {p:.1f} ms, decode {s:.3f} ms/step" for n, (p, s) in res.items()))
+    for m in models.values():
+        m.engine._decode.clear()
+    del inp_big
+    torch.cuda.empty_cache()
+    # each decode GEMM with its tail, over the weights of all layers in turn
+    m16, eng16, engq = models["16-bit"], models["16-bit"].engine, models["int8"].engine
+    eng16.set_format()
+    E, I = llama.hidden_size, llama.intermediate_size
+    L = len(m16.llm.model.layers)
+    w16 = [eng16._llama_weights(i, l, E, I) for i, l in enumerate(m16.llm.model.layers)]
+    w8 = [engq._w8_layer(i, l) for i, l in enumerate(models["int8"].llm.model.layers)]
+    cos, sin = eng16.rope_tables(64, 128, "cuda")
+    for M in batches:
+        g = torch.Generator(device="cuda").manual_seed(M)
+        x = (torch.randn((M, E), device="cuda", generator=g)).to(dtype)
+        h = (torch.randn((M, I), device="cuda", generator=g)).to(dtype)
+        rs = torch.ones((M,), device="cuda")
+        cache = torch.zeros((M, 64, 2, E), device="cuda", dtype=dtype)
+        pos = torch.tensor([3], device="cuda", dtype=torch.int32)
+        gemms = (("qkv", 0, x, dict(mode=ops.THIN_QKV, row_scale=rs, rope=(cos, sin, pos), cache=cache, t0_dev=pos)),
+                 ("o_proj", 2, x, dict(mode=ops.THIN_RES, residual=x)),
+                 ("gate_up", 1, x, dict(mode=ops.THIN_SWIGLU, row_scale=rs)),
+                 ("down_proj", 3, h, dict(mode=ops.THIN_RES, residual=x)))
+        for name, j, inp, kw in gemms:
+            kw = dict(kw)
+            mode = kw.pop("mode")
+            N, K = w16[0][j].shape
+            t16 = _gemm_us(lambda i: ops.linear_thin_fused(inp, w16[i][j], mode, **kw), L, 20)
+            t8 = _gemm_us(lambda i: ops.linear_w8_thin_fused(inp, w8[i][j], mode, **kw), L, 20)
+            b16, b8 = 2 * N * K, N * K + 4 * N
+            print(f"[bench_decode] gemm {name:9s} {N}x{K} M={M:2d}: 16-bit {t16:7.1f} us ({b16 / t16 / 1e6:.2f} TB/s, "
+                  f"{b16 / t16 / 1e6 / HBM_BPS * 1e12:.0%}); int8 {t8:7.1f} us ({b8 / t8 / 1e6:.2f} TB/s, "
+                  f"{b8 / t8 / 1e6 / HBM_BPS * 1e12:.0%}); {t16 / t8:.2f}x")
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=8)
@@ -70,14 +186,17 @@ def main():
     ap.add_argument("--top-k", type=int, default=50)
     ap.add_argument("--top-p", type=float, default=0.6)
     ap.add_argument("--repetition-penalty", type=float, default=1.0)
-    ap.add_argument("--dtype", choices=("bf16", "fp16"), default=None, help="default: fp16 with --sample, else bf16")
+    ap.add_argument("--int8", action="store_true", help="compare the 16-bit decoder with its int8-quantized twin")
+    ap.add_argument("--dtype", choices=("bf16", "fp16"), default=None, help="default: fp16 with --sample / --int8, else bf16")
     a = ap.parse_args()
     from macaw_llm_b200 import ops
     from macaw_llm_b200.modeling import MM_LLMs, MM_LLMs_Config
 
-    dtype = {"bf16": torch.bfloat16, "fp16": torch.float16}[a.dtype or ("fp16" if a.sample else "bf16")]
+    dtype = {"bf16": torch.bfloat16, "fp16": torch.float16}[a.dtype or ("fp16" if a.sample or a.int8 else "bf16")]
     (clip, whisper, llama), hyper = bench.real_configs()
     cfg = MM_LLMs_Config(clip_config=clip, whisper_config=whisper, llm_config=llama, **hyper)
+    if a.int8:
+        return _int8(a, cfg, dtype)
     model = MM_LLMs.build_random(cfg, device="cuda", dtype=dtype, seed=0)
     host = bench.synth_inputs(a.batch, a.seq_len, llama.vocab_size, 224, 3000, 1234)
     host["audios"] = None
