@@ -223,24 +223,36 @@ __device__ __forceinline__ int ld_acquire_gpu(const int* p) {
   return v;
 }
 
-__device__ __forceinline__ float tanh_approx(float x) {
+__device__ __forceinline__ float rcp_approx(float x) {
   float y;
-  asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// sigmoid(x) = 0.5 tanh(0.5 x) + 0.5: one MUFU op (tanh.approx.f32, rel. error ~2^-11 — far below the bf16 output rounding)
-__device__ __forceinline__ float sigmoid_fast(float x) { return fmaf(0.5f, tanh_approx(0.5f * x), 0.5f); }
-// exact-GELU's erf via Abramowitz-Stegun 7.1.26 (|error| <= 1.5e-7): 2 MUFU + ~10 FMA, branch-free
+// sigmoid(x) = 1 / (1 + e^-x): __expf (documented bound 2 + 1.17 |x| ulps) and rcp.approx (1 ulp), so the relative
+// error stays a few fp32 ulps where sigma is tiny (down to x ~ -87, where e^-x overflows and sigma flushes to 0).  The
+// former 0.5 tanh.approx(0.5 x) + 0.5 had an ABSOLUTE error near 2^-12, i.e. most of sigma in the negative tail, and
+// returned 0 below x ~ -16: on an H100, SiLU / SwiGLU outputs were up to 511 bf16 / 60 fp16 output roundings off and
+// quick-GELU 512 / 35 (tests/test_gemm_fp64_gpu.py, activation sweep over [-30, 30]).
+__device__ __forceinline__ float sigmoid_fast(float x) { return rcp_approx(1.0f + __expf(-x)); }
+// exact GELU 0.5 x erfc(-x / sqrt 2), with erfc(z) = t exp(-z^2 + P(t)), t = 1 / (1 + z / 2) (the Chebyshev fit of
+// Numerical Recipes' erfcc, relative error < 1.2e-7 for every z >= 0) taken at z = |x| / sqrt 2 and reflected for
+// x >= 0: no cancellation in the negative tail.  The former 0.5 x + 0.5 |x| (1 - Abramowitz-Stegun 7.1.26) cancelled
+// to nothing there (fp32 1 - erf) and that polynomial is 0.07-0.7 % off erfc for |x| in 3..7: up to 646 bf16 output
+// roundings at x = -5.5.
 __device__ __forceinline__ float gelu_erf(float x) {
   const float z = fabsf(x) * 0.70710678118654752f;
-  const float t = __frcp_rn(fmaf(0.3275911f, z, 1.0f));
-  float poly = fmaf(1.061405429f, t, -1.453152027f);
-  poly = fmaf(poly, t, 1.421413741f);
-  poly = fmaf(poly, t, -0.284496736f);
-  poly = fmaf(poly, t, 0.254829592f);
-  poly *= t;
-  const float e = 1.0f - poly * exp2f(-1.4426950408889634f * z * z);  // erf(|x| / sqrt 2)
-  return 0.5f * x + 0.5f * fabsf(x) * e;                                 // 0.5 x (1 + sign(x) erf(|x|/sqrt2))
+  const float t = __frcp_rn(fmaf(0.5f, z, 1.0f));
+  float p = fmaf(0.17087277f, t, -0.82215223f);
+  p = fmaf(p, t, 1.48851587f);
+  p = fmaf(p, t, -1.13520398f);
+  p = fmaf(p, t, 0.27886807f);
+  p = fmaf(p, t, -0.18628806f);
+  p = fmaf(p, t, 0.09678418f);
+  p = fmaf(p, t, 0.37409196f);
+  p = fmaf(p, t, 1.00002368f);
+  p = fmaf(p, t, -1.26551223f);
+  const float q = t * exp2f(1.4426950408889634f * fmaf(-z, z, p));  // erfc(|x| / sqrt 2)
+  return 0.5f * x * (x >= 0.0f ? 2.0f - q : q);
 }
 
 // bias / residual elements in the run-time activation format

@@ -84,18 +84,27 @@ def gemm_raw(*, M, N, K, A, lda, B, ldb, Cout, ldc, batch=1, a_bs=0, b_bs=0, c_b
              row_scale=None, residual=None, ldr=0, r_bs=0, r_bs2=0, res_row_mod=0, rope_cos=None, rope_sin=None,
              rope_T=0, rope_cols=0, rope_pos=None, c_trans=False, a_fp16=None, b_fp16=None, c_fp16=None,
              bias_rs=None, bias2=None, bias2_rs=None, a_mn_major=False, sumsq_out=None, rs_sumsq=None, rs_parts=0,
-             rs_eps=0.0, streamk: Optional[torch.Tensor] = None) -> None:
+             rs_eps=0.0, streamk=None, plan_only: bool = False):
     """Direct binding of mm_gemm_fwd; pointers are ints (data_ptr() + byte offsets).  Operand / output formats default to
-    the current activation format (ACT()): fp16 for an fp16 model, bf16 otherwise."""
+    the current activation format (ACT()): fp16 for an fp16 model, bf16 otherwise.  `streamk` is a workspace tensor, or
+    (address, bytes).  plan_only=True launches nothing and returns the gemm_plan() dict of exactly these arguments
+    (mm_gemm_plan: no memory is touched, so the pointers may be fake); while PLANS is a list, every launch appends its own."""
     f16 = ACT() == _F16
     a_fp16 = f16 if a_fp16 is None else a_fp16
     b_fp16 = f16 if b_fp16 is None else b_fp16
     c_fp16 = (f16 and not c_fp32) if c_fp16 is None else c_fp16
+    if isinstance(streamk, torch.Tensor):
+        streamk = (streamk.data_ptr(), streamk.numel() * streamk.element_size())
     a = GemmArgs(M, N, K, batch, batch2, A, lda, a_bs, a_bs2, B, ldb, b_bs, b_bs2, int(b_mn_major), Cout, ldc, c_bs,
                  c_bs2, int(c_fp32), epi, act, float(alpha), bias, bias_bs, row_scale, residual, ldr, r_bs, r_bs2,
                  res_row_mod, rope_cos, rope_sin, rope_T, rope_cols, rope_pos, int(c_trans), int(a_fp16), int(b_fp16), int(c_fp16),
                  bias_rs, bias2, bias2_rs, int(a_mn_major), sumsq_out, rs_sumsq, int(rs_parts), float(rs_eps),
-                 None if streamk is None else streamk.data_ptr(), 0 if streamk is None else streamk.numel() * streamk.element_size())
+                 None if streamk is None else streamk[0], 0 if streamk is None else streamk[1])
+    if plan_only or PLANS is not None:
+        plan = _plan_of(a)
+        if plan_only:
+            return plan
+        PLANS.append(plan)
     if PROFILE is None:
         _check(_lib.load().mm_gemm_fwd(C.byref(a), _stream()), "mm_gemm_fwd")
         return
@@ -125,9 +134,16 @@ def gemm_plan(*, M: int, N: int, K: int, batch: int = 1, batch2: int = 1, epi: i
               c_bs2=M * n_out * batch, c_fp32=int(c_fp32), epi=epi, act=ACT_NONE, alpha=1.0, c_trans=int(c_trans),
               a_fp16=int(fp16), b_fp16=int(fp16), c_fp16=int(fp16 and not c_fp32), a_mn_major=int(a_mn_major),
               sk_workspace=fake if streamk else None, sk_workspace_bytes=ws, **rope)
-    a = GemmArgs(**kw)
+    return _plan_of(GemmArgs(**kw))
+
+
+# While a list, gemm_raw appends the gemm_plan() dict of every launch's own arguments (what the dispatcher decided).
+PLANS = None
+
+
+def _plan_of(a: GemmArgs) -> dict:
     plan = _lib.GemmPlan()
-    _check(lib.mm_gemm_plan(C.byref(a), C.byref(plan)), "mm_gemm_plan")
+    _check(_lib.load().mm_gemm_plan(C.byref(a), C.byref(plan)), "mm_gemm_plan")
     d = {name: int(getattr(plan, name)) for name, _ in _lib.GemmPlan._fields_}
     d["fill"] = d["units"] / float(d["waves"] * d["workers"])  # share of the scheduled tile slots that carry work
     return d
