@@ -573,6 +573,40 @@ int32_t mm_dequant_rows(const mm_w8_matrix* w, void* out, int64_t ldo, void* str
 int32_t mm_gemm_w8_thin(const mm_w8_matrix* w, const void* x, int64_t ldx, int32_t M, float* part, int32_t splits,
                         int32_t ldp, void* xs_work, void* stream);
 
+/* ------------------------------------------------------------------------------------------------ FP8 (e4m3) decoder
+ * Per-row e4m3 weights AND activations for the decoder's prefill GEMMs (csrc/quant.cu, csrc/gemm_wgmma.cu).
+ *
+ * mm_quantize_rows_e4m3: x (rows, K) with row stride ldx, format x_format (0 bf16, 1 fp16, 2 fp32), optional gain [K] in
+ *   the activation format -> v = fp32(x) * fp32(g) (v = fp32(x) without gain),
+ *   s[r] = fp32(max_k |v[r][k]|) / 448 (IEEE division),  q[r][k] = e4m3(v[r][k] / s[r]) (IEEE division, round to nearest
+ *   even, saturated to +-448: cvt.rn.satfinite), q = 0 where s = 0.  q (rows, K) bytes with row stride ldq; K % 16 == 0,
+ *   x, gain and q 16-byte aligned, ldx a whole number of 16-byte units, ldq % 16 == 0.  Deterministic, no host
+ *   synchronisation.
+ *
+ * mm_gemm_e4m3_fwd: mm_gemm_fwd's epilogues on an e4m3 product,
+ *   C = epilogue((acc[m][n] * a_scale[m]) * s_w[n]),  acc = sum_k qa[m][k] qw[n][k] (fp32),
+ *   with A = args->A the e4m3 activation rows (M, K) (row stride args->lda bytes, lda % 16 == 0) and the weight the e4m3
+ *   mm_w8_matrix `w` (its q[] hold e4m3 bytes; gathered through w.chunks, no fused copy; w.gain must be null; w.N ==
+ *   args->N, w.K == args->K).  Every other field of args means what it means for mm_gemm_fwd, except: args->B / ldb /
+ *   a_fp16 / b_fp16 and the stream-K workspace are ignored; no batching, no c_trans, no MN-major operands; K % 128 == 0,
+ *   N % 128 == 0.  The main loop accumulates each 128-deep k-block in a fresh register tile and adds it to fp32 master
+ *   accumulators (promotion every four k32 MMAs); `unpromoted` = 1 lets the MMAs accumulate all of K in place instead
+ *   (a comparison instance for tests).  The variant is always MM_GEMM_KERNEL_CONSUMER_EPILOGUE with block_n = 128.
+ * mm_gemm_e4m3_plan: the launch mm_gemm_e4m3_fwd would make for these arguments (no memory is touched, no GPU needed).
+ * mm_gemm_e4m3_thin: mm_gemm_w8_thin with e4m3 weight bytes (converted exactly to the activation format in registers):
+ *   part[s][n][m] = s_n * sum_{k in slice s} e4m3(q[n][k]) x~[m][k], x~ = round16(x[m][k] g[k]); same arguments. */
+typedef struct mm_gemm_e4m3_args {
+  const float* a_scale;   /* [M] fp32 per-row scales of A */
+  mm_w8_matrix w;         /* the weight: e4m3 sources, per-row fp32 scales, chunk table */
+  int32_t unpromoted;
+} mm_gemm_e4m3_args;
+int32_t mm_quantize_rows_e4m3(const void* x, int64_t ldx, int32_t x_format, int32_t rows, int32_t K, const void* gain,
+                              uint8_t* q, int64_t ldq, float* scale, void* stream);
+int32_t mm_gemm_e4m3_fwd(const mm_gemm_args* args, const mm_gemm_e4m3_args* e, void* stream);
+int32_t mm_gemm_e4m3_plan(const mm_gemm_args* args, const mm_gemm_e4m3_args* e, mm_gemm_schedule* plan);
+int32_t mm_gemm_e4m3_thin(const mm_w8_matrix* w, const void* x, int64_t ldx, int32_t M, float* part, int32_t splits,
+                          int32_t ldp, void* xs_work, void* stream);
+
 /* ------------------------------------------------------------------------------------------------ gradient all-reduce
  * The one collective of the path: the data-parallel gradient all-reduce of the training step (reference: DeepSpeed ZeRO-3
  * reduce-scatter / all-gather, configs/deepspeed_config.json:22-41; north_star: "a single NCCL all-reduce on gradients").

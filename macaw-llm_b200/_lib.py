@@ -103,6 +103,12 @@ class W8Matrix(C.Structure):
                 ("gain", c_vp)]
 
 
+class GemmE4m3Args(C.Structure):
+    """Mirror of `mm_gemm_e4m3_args` (include/macaw_b200.h)."""
+
+    _fields_ = [("a_scale", c_vp), ("w", W8Matrix), ("unpromoted", c_i32)]
+
+
 class LossScaleState(C.Structure):
     """Mirror of `mm_loss_scale_state` (include/macaw_b200.h): 12 four-byte fields."""
 
@@ -232,6 +238,10 @@ SIGNATURES = {
     "mm_quantize_rows_int8": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_i32, c_vp, c_vp, c_vp]),
     "mm_dequant_rows": (c_i32, [C.POINTER(W8Matrix), c_vp, c_i64, c_vp]),
     "mm_gemm_w8_thin": (c_i32, [C.POINTER(W8Matrix), c_vp, c_i64, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp]),
+    "mm_quantize_rows_e4m3": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_i32, c_vp, c_vp, c_i64, c_vp, c_vp]),
+    "mm_gemm_e4m3_fwd": (c_i32, [C.POINTER(GemmArgs), C.POINTER(GemmE4m3Args), c_vp]),
+    "mm_gemm_e4m3_plan": (c_i32, [C.POINTER(GemmArgs), C.POINTER(GemmE4m3Args), C.POINTER(GemmPlan)]),
+    "mm_gemm_e4m3_thin": (c_i32, [C.POINTER(W8Matrix), c_vp, c_i64, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp]),
 }
 
 # Nullable pointers added to an entry after it first shipped, just before its final `stream` argument: a Python call may

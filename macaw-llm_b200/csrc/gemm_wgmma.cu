@@ -986,6 +986,187 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 }
 
+// ------------------------------------------------------------------------------------------------ e4m3 main loop
+// C = epilogue((acc * s_x[m]) * s_w[n]) with acc = sum_k q_x[m][k] q_w[n][k] over per-row e4m3 activations and weights
+// (mm_gemm_e4m3_fwd).  128 x 128 tiles; a k-block is 128 e4m3 = 128 B deep, so the 128B-swizzled TMA boxes, the 32 KiB
+// stage and its descriptors are those of the 16-bit kernel at BN = 128, and each k-block is four m64n128k32 MMAs.
+//
+// Promoted accumulation (PROMOTE): the four MMAs of a k-block accumulate into a fresh register tile (scale-d = 0 on the
+// first), which is then added to the fp32 master accumulators with FADD, so the MMA's own accumulator only ever sums 128
+// products.  The consumer waits for each k-block's MMAs before promoting; the other warpgroup's MMAs fill the tensor
+// cores meanwhile.  Master plus promoted tiles are 128 registers per thread: the 288-thread consumer-epilogue block (up to
+// 224 per thread) holds them without spills, the epilogue-warpgroup block (152 for the consumers) would not, so this is the
+// one variant.  No stream-K, no tile pairs.
+//
+// The B tile of a 128-row N block is four 32-row chunks, each loaded from the tensor map of its source (chunk table of the
+// mm_w8_matrix, as the int8 decode kernel reads it): the fused [q; k; v] and [gate | up] weights are never copied.
+// Everything after the main loop is the 16-bit kernel's: tile schedule, staging tile, gemm_epilogue<128, EPI>.
+struct E4m3P {
+  const float* a_scale;
+  const float* w_scale[MM_W8_MAX_SRC];
+  int w_rows[MM_W8_MAX_SRC];
+  const int32_t* chunks;
+};
+
+__device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar, void* dst, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+               ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+               : "memory");
+}
+
+// scale of fused weight row n (0 for a chunk-table entry that does not name 32 rows of a present source)
+__device__ __forceinline__ float e4m3_w_scale(const E4m3P& e, int n) {
+  const int2 c = reinterpret_cast<const int2*>(e.chunks)[n >> 5];
+  const int rows = c.x == 0 ? e.w_rows[0] : c.x == 1 ? e.w_rows[1] : e.w_rows[2];
+  const float* s = c.x == 0 ? e.w_scale[0] : c.x == 1 ? e.w_scale[1] : e.w_scale[2];
+  if (c.x < 0 || c.x >= MM_W8_MAX_SRC || s == nullptr || c.y < 0 || c.y + 32 > rows) return 0.f;
+  return __ldg(s + c.y + (n & 31));
+}
+
+constexpr int kE4m3BlockK = 128;  // e4m3 elements per k-block (128 B rows)
+
+template <int EPI, bool PROMOTE>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_e4m3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB0,
+                 const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2, const GemmKParams p,
+                 const E4m3P e) {
+  constexpr int BN = kMaxBN;
+  constexpr int STAGES = gemm_stages(BN);
+  constexpr uint32_t B_BYTES = BN * kE4m3BlockK;
+  static_assert(B_BYTES == BN * kBlockK * 2 && kABytes == kBlockM * kE4m3BlockK, "e4m3 stage = the 16-bit stage");
+  constexpr int LDS = gemm_stage_ld(BN);
+  extern __shared__ uint8_t smem_raw[];
+  const GemmSmem sm = gemm_smem<STAGES, B_BYTES, BN>(smem_raw);
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int worker = static_cast<int>(blockIdx.x);
+  const int n_workers = static_cast<int>(gridDim.x);
+  const int m_units = p.m_tiles;
+  const int total_tiles = m_units * p.n_tiles;
+
+  if (warp == kProducerWarp && elect_one()) {
+    gemm_prologue<STAGES, false>(sm, &tmA, &tmB0);
+    tma_prefetch_desc(&tmB1);
+    tma_prefetch_desc(&tmB2);
+  }
+  __syncthreads();
+  griddep_launch();
+  griddep_wait();
+
+  if (warp == kProducerWarp) {
+    // ------------------------------------------------------------------ TMA producer
+    if (elect_one()) {
+      int stage = 0;
+      uint32_t phase = 0;
+      GemmWork wk;
+      for (int it = 0; gemm_work(p, worker, n_workers, total_tiles, it, wk); ++it) {
+        const TileCoord t = tile_coord(wk.tile, p, m_units);
+        const CUtensorMap* bm[4];
+        int brow[4];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          const int2 ch = reinterpret_cast<const int2*>(e.chunks)[t.n_blk * 4 + c];
+          bm[c] = ch.x == 0 ? &tmB0 : ch.x == 1 ? &tmB1 : &tmB2;
+          brow[c] = ch.y;
+        }
+        for (int kb = wk.kb0; kb < wk.kb1; ++kb) {
+          mbar_wait(&sm.empty_bar[stage], phase ^ 1);
+          mbar_arrive_expect_tx(&sm.full_bar[stage], kABytes + B_BYTES);
+          tma_load_2d(&tmA, &sm.full_bar[stage], sm.sA + stage * kABytes, kb * kE4m3BlockK, t.m_blk * kBlockM);
+#pragma unroll
+          for (int c = 0; c < 4; ++c)
+            tma_load_2d(bm[c], &sm.full_bar[stage], sm.sB + stage * B_BYTES + c * (32 * kE4m3BlockK), kb * kE4m3BlockK,
+                        brow[c]);
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers: main loop, then the epilogue
+  const int q = warp & 3;
+  const float* srow = sm.sC + (q * 32 + lane) * LDS;
+  const int wg = warp >> 2;
+  int stage = 0;
+  uint32_t phase = 0;
+  GemmWork wk;
+  for (int it = 0; gemm_work(p, worker, n_workers, total_tiles, it, wk); ++it) {
+    const TileCoord t = tile_coord(wk.tile, p, m_units);
+    {
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int kb = wk.kb0; kb < wk.kb1; ++kb) {
+        mbar_wait(&sm.full_bar[stage], phase);
+        const uint64_t a_desc = make_sdesc_sw128(smem_u32(sm.sA + stage * kABytes) + wg * 8192, 16, 1024);
+        const uint64_t b_desc = make_sdesc_sw128(smem_u32(sm.sB + stage * B_BYTES), 16, 1024);
+        if constexpr (PROMOTE) {
+          float part[BN / 2];
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < kE4m3BlockK / 32; ++kk)  // k32 step = 32 B inside the swizzle atom
+            wgmma_e4m3_n128(part, a_desc + static_cast<uint64_t>(kk * 2), b_desc + static_cast<uint64_t>(kk * 2),
+                            kk > 0 ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<0>();
+          fence_regs(part);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&sm.empty_bar[stage]);
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+        } else {
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < kE4m3BlockK / 32; ++kk)
+            wgmma_e4m3_n128(acc, a_desc + static_cast<uint64_t>(kk * 2), b_desc + static_cast<uint64_t>(kk * 2), 1u);
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (prev >= 0) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&sm.empty_bar[prev]);
+          }
+          prev = stage;
+        }
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      if constexpr (!PROMOTE) {
+        wgmma_wait<0>();
+        fence_regs(acc);
+        __syncwarp();
+        if (lane == 0 && prev >= 0) mbar_arrive(&sm.empty_bar[prev]);
+      }
+      // acc * s_x[m] * s_w[n] (fixed fp32 order) -> staging tile; the previous tile's epilogue must be done reading it
+      const int r0 = t.m_blk * kBlockM + wg * 64 + q * 16 + (lane >> 2);
+      const float sx0 = r0 < p.M ? __ldg(e.a_scale + r0) : 0.f;
+      const float sx1 = r0 + 8 < p.M ? __ldg(e.a_scale + r0 + 8) : 0.f;
+      const int n0 = t.n_blk * BN + 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const float sw0 = e4m3_w_scale(e, n0 + 8 * j), sw1 = e4m3_w_scale(e, n0 + 8 * j + 1);
+        acc[4 * j] = acc[4 * j] * sx0 * sw0;
+        acc[4 * j + 1] = acc[4 * j + 1] * sx0 * sw1;
+        acc[4 * j + 2] = acc[4 * j + 2] * sx1 * sw0;
+        acc[4 * j + 3] = acc[4 * j + 3] * sx1 * sw1;
+      }
+      consumer_sync();
+      stage_acc<BN>(sm.sC, acc, 0, wg, q, lane);
+      consumer_sync();
+    }
+    const int half = warp >> 2;
+    const float rs = epi_row_scale(p, t, t.m_blk * kBlockM + q * 32 + lane);
+    gemm_epilogue<BN, EPI>(p, t, wk, srow, rs, q, lane, half, warp, worker, n_workers);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
@@ -1289,6 +1470,133 @@ extern "C" int32_t mm_gemm_overlap_mode(int32_t mode) {
 
 extern "C" int64_t mm_gemm_streamk_workspace_bytes(void) {
   return 8192 + static_cast<int64_t>(num_sms()) * kBlockM * kMaxBN * 4;
+}
+
+// ------------------------------------------------------------------------------------------------ e4m3 host side
+namespace mm {
+// e4m3 2-D map {inner (bytes), rows}; 128B swizzle; box {128, box_rows}; rows past `rows` and columns past `inner` read 0
+static int make_map_e4m3(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t rows, uint64_t ld, uint32_t box_rows) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (fn == nullptr) {
+    set_error("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
+    return 1;
+  }
+  cuuint64_t dims[2] = {inner, rows};
+  cuuint64_t strides[1] = {ld};
+  cuuint32_t box[2] = {static_cast<cuuint32_t>(kE4m3BlockK), box_rows}, estr[2] = {1, 1};
+  const CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("mm_gemm_e4m3_fwd: cuTensorMapEncodeTiled failed (%d): ptr=%p %llu x %llu ld=%llu", static_cast<int>(r), ptr,
+              (unsigned long long)rows, (unsigned long long)inner, (unsigned long long)ld);
+    return 1;
+  }
+  return 0;
+}
+
+// The e4m3 operands are checked here; the epilogue arguments by plan_gemm() on the 16-bit view of the same problem (A and
+// B as if K-major 16-bit with lda = ldb = K), whose decisions are then replaced: 128-wide tiles, 128-deep k-blocks, no
+// stream-K, the consumer-epilogue kernel.
+static int plan_gemm_e4m3(const mm_gemm_args* a, const mm_gemm_e4m3_args* e, GemmLaunch& L) {
+  MM_REQUIRE(a != nullptr && e != nullptr, "mm_gemm_e4m3_fwd: null args");
+  MM_REQUIRE(a->M > 0 && a->N > 0 && a->K > 0, "mm_gemm_e4m3_fwd: bad shape M=%d N=%d K=%d", a->M, a->N, a->K);
+  MM_REQUIRE(a->K % kE4m3BlockK == 0, "mm_gemm_e4m3_fwd: K %% 128 == 0 required (K=%d)", a->K);
+  MM_REQUIRE(a->N % kMaxBN == 0, "mm_gemm_e4m3_fwd: N %% 128 == 0 required (N=%d)", a->N);
+  MM_REQUIRE(a->batch == 1 && a->batch2 <= 1 && !a->c_trans && !a->a_mn_major && !a->b_mn_major,
+             "mm_gemm_e4m3_fwd: no batching, c_trans or MN-major operands");
+  MM_REQUIRE(a->A != nullptr && (reinterpret_cast<uintptr_t>(a->A) & 15) == 0 && a->lda >= a->K && a->lda % 16 == 0,
+             "mm_gemm_e4m3_fwd: A must be 16-byte aligned with lda >= K and lda %% 16 == 0 (lda=%lld)", (long long)a->lda);
+  MM_REQUIRE(e->a_scale != nullptr, "mm_gemm_e4m3_fwd: null A scales");
+  MM_REQUIRE(!e->unpromoted || a->epi == MM_EPI_STD,
+             "mm_gemm_e4m3_fwd: the unpromoted comparison instance has the standard epilogue only");
+  const mm_w8_matrix& w = e->w;
+  MM_REQUIRE(w.N == a->N && w.K == a->K, "mm_gemm_e4m3_fwd: weight is %d x %d, the problem needs %d x %d", w.N, w.K, a->N,
+             a->K);
+  MM_REQUIRE(w.chunks != nullptr && (reinterpret_cast<uintptr_t>(w.chunks) & 15) == 0,
+             "mm_gemm_e4m3_fwd: chunk table (16-byte aligned)");
+  MM_REQUIRE(w.gain == nullptr, "mm_gemm_e4m3_fwd: the weight's gain must be null (apply it when quantizing A)");
+  MM_REQUIRE(w.q[0] != nullptr, "mm_gemm_e4m3_fwd: weight source 0");
+  for (int j = 0; j < MM_W8_MAX_SRC; ++j) {
+    MM_REQUIRE(w.q[j] == nullptr || (reinterpret_cast<uintptr_t>(w.q[j]) & 15) == 0,
+               "mm_gemm_e4m3_fwd: weight source %d must be 16-byte aligned", j);
+    MM_REQUIRE(w.q[j] == nullptr || (w.scale[j] != nullptr && w.rows[j] > 0 && w.rows[j] % 32 == 0),
+               "mm_gemm_e4m3_fwd: weight source %d needs non-null scales and a positive multiple of 32 rows", j);
+  }
+  mm_gemm_args v = *a;
+  v.B = w.q[0];
+  v.lda = v.ldb = a->K;
+  v.a_fp16 = v.b_fp16 = 0;
+  v.sk_workspace = nullptr;
+  v.sk_workspace_bytes = 0;
+  if (int rc = plan_gemm(&v, L)) return rc;
+  GemmKParams& p = L.p;
+  const int sms = num_sms();
+  p.n_tiles = a->N / kMaxBN;
+  p.num_k = a->K / kE4m3BlockK;
+  {
+    const long long unit_bytes = (long long)kBlockM * a->K;
+    long long g = ((16LL << 20) + unit_bytes / 2) / unit_bytes;
+    p.group_m = static_cast<int>(g < 2 ? 2 : (g > 32 ? 32 : g));
+  }
+  p.sk_tiles = 0; p.sk_first = 0; p.sk_ws = nullptr; p.sk_flags = nullptr;
+  const long long tiles = (long long)p.m_tiles * p.n_tiles;
+  mm_gemm_schedule& s = L.s;
+  s.block_n = kMaxBN; s.m_tiles = p.m_tiles; s.n_tiles = p.n_tiles; s.k_blocks = p.num_k; s.group_m = p.group_m;
+  s.units = tiles; s.workers = sms; s.waves = static_cast<int>((tiles + sms - 1) / sms);
+  s.streamk_tiles = 0; s.vectorised_epilogue = p.vec_ok;
+  s.kernel = MM_GEMM_KERNEL_CONSUMER_EPILOGUE;
+  s.threads = kGemmThreads;
+  s.smem_bytes = static_cast<int32_t>(gemm_smem_bytes(gemm_stages(kMaxBN), kMaxBN * kE4m3BlockK, kMaxBN));
+  s.grid = static_cast<int>(tiles < sms ? tiles : sms);
+  return 0;
+}
+
+template <int EPI, bool PROMOTE>
+static int launch_e4m3(const GemmLaunch& L, const CUtensorMap (&tm)[4], const E4m3P& e, cudaStream_t st) {
+  auto kern = &gemm_e4m3_kernel<EPI, PROMOTE>;
+  static bool attr_set[kMaxDevices] = {};
+  if (int rc = ensure_smem_attr(kern, L.s.smem_bytes, attr_set, "mm_gemm_e4m3_fwd")) return rc;
+  cudaError_t err = launch_kernel(kern, dim3(L.s.grid), dim3(L.s.threads), L.s.smem_bytes, st, 1, tm[0], tm[1], tm[2], tm[3],
+                                  L.p, e);
+  if (err != cudaSuccess) {
+    set_error("mm_gemm_e4m3_fwd: launch failed: %s", cudaGetErrorString(err));
+    return 2;
+  }
+  return check_launch("mm_gemm_e4m3_fwd");
+}
+}  // namespace mm
+
+extern "C" int32_t mm_gemm_e4m3_plan(const mm_gemm_args* a, const mm_gemm_e4m3_args* e, mm_gemm_schedule* plan) {
+  MM_REQUIRE(plan != nullptr, "mm_gemm_e4m3_plan: null plan");
+  GemmLaunch L;
+  if (int rc = plan_gemm_e4m3(a, e, L)) return rc;
+  *plan = L.s;
+  return 0;
+}
+
+extern "C" int32_t mm_gemm_e4m3_fwd(const mm_gemm_args* a, const mm_gemm_e4m3_args* e, void* stream) {
+  GemmLaunch L;
+  if (int rc = plan_gemm_e4m3(a, e, L)) return rc;
+  CUtensorMap tm[4];
+  if (make_map_e4m3(&tm[0], a->A, a->K, a->M, a->lda, kBlockM)) return 1;
+  const mm_w8_matrix& w = e->w;
+  for (int j = 0; j < MM_W8_MAX_SRC; ++j) {
+    const int src = w.q[j] != nullptr ? j : 0;  // absent sources get source 0's map (the chunk table never names them)
+    if (make_map_e4m3(&tm[1 + j], w.q[src], w.K, w.rows[src], w.K, 32)) return 1;
+  }
+  E4m3P ep = {};
+  ep.a_scale = e->a_scale;
+  for (int j = 0; j < MM_W8_MAX_SRC; ++j) {
+    ep.w_scale[j] = w.q[j] != nullptr ? w.scale[j] : nullptr;
+    ep.w_rows[j] = w.q[j] != nullptr ? w.rows[j] : 0;
+  }
+  ep.chunks = w.chunks;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  if (e->unpromoted) return launch_e4m3<MM_EPI_STD, false>(L, tm, ep, st);
+  if (a->epi == MM_EPI_ROPE) return launch_e4m3<MM_EPI_ROPE, true>(L, tm, ep, st);
+  if (a->epi == MM_EPI_SWIGLU) return launch_e4m3<MM_EPI_SWIGLU, true>(L, tm, ep, st);
+  return launch_e4m3<MM_EPI_STD, true>(L, tm, ep, st);
 }
 
 

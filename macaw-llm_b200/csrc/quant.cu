@@ -22,6 +22,7 @@
 #include "common.cuh"
 #include "ptx.cuh"
 #include "../../include/macaw_b200.h"
+#include <cuda_fp8.h>
 
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
 
@@ -97,6 +98,21 @@ __device__ __forceinline__ void cvt_s8x4(uint32_t w, uint32_t& lo, uint32_t& hi)
   }
 }
 
+// four e4m3 (bytes 0..3 of w) -> two pairs in the 16-bit format, as cvt_s8x4.  e4m3 -> f16 is exact (cvt.rn.f16x2.e4m3x2),
+// and so is f16 -> f32 -> bf16 for every e4m3 value (3 significand bits, exponents -9 .. 8)
+template <bool F16>
+__device__ __forceinline__ void cvt_e4m3x4(uint32_t w, uint32_t& lo, uint32_t& hi) {
+  const __half2_raw a = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(w & 0xFFFFu), __NV_E4M3);
+  const __half2_raw b = __nv_cvt_fp8x2_to_halfraw2(static_cast<__nv_fp8x2_storage_t>(w >> 16), __NV_E4M3);
+  if constexpr (F16) {
+    lo = static_cast<uint32_t>(a.x) | (static_cast<uint32_t>(a.y) << 16);
+    hi = static_cast<uint32_t>(b.x) | (static_cast<uint32_t>(b.y) << 16);
+  } else {
+    lo = pack_bf16x2(__half2float(__ushort_as_half(a.x)), __half2float(__ushort_as_half(a.y)));
+    hi = pack_bf16x2(__half2float(__ushort_as_half(b.x)), __half2float(__ushort_as_half(b.y)));
+  }
+}
+
 template <bool F16, int MN>
 __device__ __forceinline__ void wgmma_w8(float (&d)[MN / 2], const uint32_t (&a)[4], uint64_t b) {
   if constexpr (MN == 8) wgmma_rs_n8<F16, 0>(d, a, b, 1u);
@@ -131,7 +147,8 @@ __global__ void __launch_bounds__(256) w8_xprep_kernel(const bf16* x, long long 
   xs[static_cast<long long>(m) * Kp + lc] = stv<F16>(v);
 }
 
-template <bool F16, int MN, bool XS>
+// FP8: the weight bytes are e4m3 (mm_gemm_e4m3_thin), else int8
+template <bool F16, int MN, bool XS, bool FP8>
 __global__ void __launch_bounds__(kThreads) w8_thin_kernel(const __grid_constant__ CUtensorMap tm0,
                                                            const __grid_constant__ CUtensorMap tm1,
                                                            const __grid_constant__ CUtensorMap tm2,
@@ -253,8 +270,13 @@ __global__ void __launch_bounds__(kThreads) w8_thin_kernel(const __grid_constant
       const uint32_t w1[4] = {w[b][1].x, w[b][1].y, w[b][1].z, w[b][1].w};
 #pragma unroll
       for (int t = 0; t < 4; ++t) {
-        cvt_s8x4<F16>(w0[t], af[b][t][0], af[b][t][2]);
-        cvt_s8x4<F16>(w1[t], af[b][t][1], af[b][t][3]);
+        if constexpr (FP8) {
+          cvt_e4m3x4<F16>(w0[t], af[b][t][0], af[b][t][2]);
+          cvt_e4m3x4<F16>(w1[t], af[b][t][1], af[b][t][3]);
+        } else {
+          cvt_s8x4<F16>(w0[t], af[b][t][0], af[b][t][2]);
+          cvt_s8x4<F16>(w1[t], af[b][t][1], af[b][t][3]);
+        }
       }
       wgmma_fence();
       const uint32_t baddr = XS ? smem_u32(st + kStageBytes) + b * (MN * 128) : xs_addr + (2 * it + b) * (MN * 128);
@@ -318,6 +340,68 @@ __global__ void __launch_bounds__(256) quantize_rows_kernel(const void* w, long 
     int v = 0;
     if (s != 0.f) v = max(-127, min(127, __float2int_rn(__fdiv_rn(ld_w<FMT>(w, base + k), s))));
     qr[k] = static_cast<int8_t>(v);
+  }
+}
+
+// ---- per-row e4m3 quantization of activations or weights: one CTA per row, eight consecutive columns per thread and step
+// (16-byte loads).  v = x g is recomputed in fp32 by both passes (the second reads the row from L1 / L2) and never rounded
+// to 16 bits; four cvt.rn.satfinite.e4m3x2 per step, one 8-byte store.
+template <int FMT>
+__device__ __forceinline__ void ld8(const void* x, long long i, float (&f)[8]) {
+  if constexpr (FMT == 2) {
+    const float4 a = *reinterpret_cast<const float4*>(static_cast<const float*>(x) + i);
+    const float4 b = *reinterpret_cast<const float4*>(static_cast<const float*>(x) + i + 4);
+    f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
+  } else {
+    unpack8t<FMT == 1>(*reinterpret_cast<const uint4*>(static_cast<const uint16_t*>(x) + i), f);
+  }
+}
+
+template <int FMT, bool GF16>
+__global__ void __launch_bounds__(256) quantize_e4m3_kernel(const void* x, long long ldx, int K, const uint16_t* gain,
+                                                            uint8_t* q, long long ldq, float* scale) {
+  __shared__ float red[8];
+  const long long row = blockIdx.x;
+  const long long base = row * ldx;
+  griddep_launch();
+  griddep_wait();
+  auto val8 = [&](int k, float (&v)[8]) {
+    ld8<FMT>(x, base + k, v);
+    if (gain != nullptr) {
+      float g[8];
+      unpack8t<GF16>(*reinterpret_cast<const uint4*>(gain + k), g);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) v[e] *= g[e];
+    }
+  };
+  float mx = 0.f;
+  for (int k = 8 * threadIdx.x; k < K; k += 8 * 256) {
+    float v[8];
+    val8(k, v);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) mx = fmaxf(mx, fabsf(v[e]));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
+  __syncthreads();
+  mx = red[0];
+#pragma unroll
+  for (int i = 1; i < 8; ++i) mx = fmaxf(mx, red[i]);
+  const float s = __fdiv_rn(mx, 448.0f);
+  if (threadIdx.x == 0) scale[row] = s;
+  uint8_t* qr = q + row * ldq;
+  for (int k = 8 * threadIdx.x; k < K; k += 8 * 256) {
+    uint32_t w[4] = {0u, 0u, 0u, 0u};
+    if (s != 0.f) {
+      float v[8];
+      val8(k, v);
+#pragma unroll
+      for (int e = 0; e < 4; ++e)
+        w[e] = __nv_cvt_float2_to_fp8x2(make_float2(__fdiv_rn(v[2 * e], s), __fdiv_rn(v[2 * e + 1], s)), __NV_SATFINITE,
+                                        __NV_E4M3);
+    }
+    *reinterpret_cast<uint2*>(qr + k) = make_uint2(w[0] | (w[1] << 16), w[2] | (w[3] << 16));
   }
 }
 
@@ -424,28 +508,28 @@ int fail_launch(cudaError_t e) {
   return 2;
 }
 
-template <bool F16, int MN, bool XS>
+template <bool F16, int MN, bool XS, bool FP8>
 int launch_w8(const CUtensorMap (&tm)[MM_W8_MAX_SRC + 1], const W8P& p, cudaStream_t st) {
   const int ns = (p.K + kStageK - 1) / kStageK;
   const int longest = (ns + p.splits - 1) / p.splits;
   const size_t smem = 1024 + static_cast<size_t>(stages<XS>()) * stage_bytes<XS, MN>() +
                       (XS ? 0 : static_cast<size_t>(2 * longest) * MN * 128) + 2 * stages<XS>() * 8;
   static bool attr[kMaxDevices];
-  if (int rc = ensure_smem_attr(w8_thin_kernel<F16, MN, XS>, smem_max<XS, MN>(), attr, "mm_gemm_w8_thin")) return rc;
-  const cudaError_t e = launch_kernel(w8_thin_kernel<F16, MN, XS>, dim3(p.N / kRows, p.splits), dim3(kThreads), smem, st, 1,
+  if (int rc = ensure_smem_attr(w8_thin_kernel<F16, MN, XS, FP8>, smem_max<XS, MN>(), attr, "mm_gemm_w8_thin")) return rc;
+  const cudaError_t e = launch_kernel(w8_thin_kernel<F16, MN, XS, FP8>, dim3(p.N / kRows, p.splits), dim3(kThreads), smem, st, 1,
                                       tm[0], tm[1], tm[2], tm[3], p);
   if (e != cudaSuccess) return fail_launch(e);
   return check_launch("mm_gemm_w8_thin");
 }
 
 // staged x~ when the longest slice's x~ fits MM_W8_XS_BYTES, else streamed (x~ written first by w8_xprep_kernel)
-template <bool F16, int MN>
+template <bool F16, int MN, bool FP8>
 int launch_w8_mode(CUtensorMap (&tm)[MM_W8_MAX_SRC + 1], const W8P& p, bf16* xs_work, cudaStream_t st) {
   const int ns = (p.K + kStageK - 1) / kStageK;
   const int longest = (ns + p.splits - 1) / p.splits;
   if (static_cast<long long>(2 * longest) * MN * 128 <= MM_W8_XS_BYTES) {
     tm[MM_W8_MAX_SRC] = tm[0];  // unused
-    return launch_w8<F16, MN, false>(tm, p, st);
+    return launch_w8<F16, MN, false, FP8>(tm, p, st);
   }
   const int Kp = ns * kStageK;
   if (int rc = make_map_2d(&tm[MM_W8_MAX_SRC], CU_TENSOR_MAP_DATA_TYPE_UINT16, xs_work, Kp, p.M, 2ull * Kp, 64, MN)) return rc;
@@ -453,16 +537,16 @@ int launch_w8_mode(CUtensorMap (&tm)[MM_W8_MAX_SRC + 1], const W8P& p, bf16* xs_
                                       p.gain, p.K, Kp, xs_work);
   if (e != cudaSuccess) return fail_launch(e);
   if (int rc = check_launch("mm_gemm_w8_thin")) return rc;
-  return launch_w8<F16, MN, true>(tm, p, st);
+  return launch_w8<F16, MN, true, FP8>(tm, p, st);
 }
 
-template <bool F16>
+template <bool F16, bool FP8>
 int dispatch_w8(CUtensorMap (&tm)[MM_W8_MAX_SRC + 1], const W8P& p, bf16* xs_work, cudaStream_t st) {
   switch (mn_of(p.M)) {
-    case 8: return launch_w8_mode<F16, 8>(tm, p, xs_work, st);
-    case 16: return launch_w8_mode<F16, 16>(tm, p, xs_work, st);
-    case 32: return launch_w8_mode<F16, 32>(tm, p, xs_work, st);
-    default: return launch_w8_mode<F16, 64>(tm, p, xs_work, st);
+    case 8: return launch_w8_mode<F16, 8, FP8>(tm, p, xs_work, st);
+    case 16: return launch_w8_mode<F16, 16, FP8>(tm, p, xs_work, st);
+    case 32: return launch_w8_mode<F16, 32, FP8>(tm, p, xs_work, st);
+    default: return launch_w8_mode<F16, 64, FP8>(tm, p, xs_work, st);
   }
 }
 
@@ -500,15 +584,18 @@ extern "C" int32_t mm_dequant_rows(const mm_w8_matrix* w, void* out, int64_t ldo
   return check_launch("mm_dequant_rows");
 }
 
-extern "C" int32_t mm_gemm_w8_thin(const mm_w8_matrix* w, const void* x, int64_t ldx, int32_t M, float* part, int32_t splits,
-                                   int32_t ldp, void* xs_work, void* stream) {
-  if (int rc = check_matrix(w, "mm_gemm_w8_thin")) return rc;
-  MM_REQUIRE(M >= 1 && M <= 64, "mm_gemm_w8_thin: M must be in [1, 64] (got %d)", M);
-  MM_REQUIRE(x != nullptr && al16(x) && ldx >= w->K && ldx % 8 == 0, "mm_gemm_w8_thin: x (16-byte aligned, ldx >= K, ldx %% 8 == 0)");
-  MM_REQUIRE(part != nullptr && al16(part) && ldp >= M && ldp % 2 == 0, "mm_gemm_w8_thin: part (16-byte aligned, ldp >= M, even)");
-  MM_REQUIRE(xs_work != nullptr && al16(xs_work), "mm_gemm_w8_thin: xs_work (16-byte aligned)");
+// mm_gemm_w8_thin and mm_gemm_e4m3_thin: one kernel family, templated on the weight element
+template <bool FP8>
+static int32_t gemm_thin(const mm_w8_matrix* w, const void* x, int64_t ldx, int32_t M, float* part, int32_t splits,
+                         int32_t ldp, void* xs_work, void* stream) {
+  const char* what = FP8 ? "mm_gemm_e4m3_thin" : "mm_gemm_w8_thin";
+  if (int rc = check_matrix(w, what)) return rc;
+  MM_REQUIRE(M >= 1 && M <= 64, "%s: M must be in [1, 64] (got %d)", what, M);
+  MM_REQUIRE(x != nullptr && al16(x) && ldx >= w->K && ldx % 8 == 0, "%s: x (16-byte aligned, ldx >= K, ldx %% 8 == 0)", what);
+  MM_REQUIRE(part != nullptr && al16(part) && ldp >= M && ldp % 2 == 0, "%s: part (16-byte aligned, ldp >= M, even)", what);
+  MM_REQUIRE(xs_work != nullptr && al16(xs_work), "%s: xs_work (16-byte aligned)", what);
   const int ns = (w->K + kStageK - 1) / kStageK;
-  MM_REQUIRE(splits >= 1 && splits <= ns, "mm_gemm_w8_thin: splits must be in [1, %d] (got %d)", ns, splits);
+  MM_REQUIRE(splits >= 1 && splits <= ns, "%s: splits must be in [1, %d] (got %d)", what, ns, splits);
   CUtensorMap tm[MM_W8_MAX_SRC + 1] = {};
   for (int j = 0; j < MM_W8_MAX_SRC; ++j) {
     const int src = w->q[j] != nullptr ? j : 0;  // unused sources get source 0's map
@@ -522,5 +609,38 @@ extern "C" int32_t mm_gemm_w8_thin(const mm_w8_matrix* w, const void* x, int64_t
   p.splits = splits;
   p.ldp = ldp;
   bf16* xw = static_cast<bf16*>(xs_work);
-  return act_f16() ? dispatch_w8<true>(tm, p, xw, ST(stream)) : dispatch_w8<false>(tm, p, xw, ST(stream));
+  return act_f16() ? dispatch_w8<true, FP8>(tm, p, xw, ST(stream)) : dispatch_w8<false, FP8>(tm, p, xw, ST(stream));
+}
+
+extern "C" int32_t mm_gemm_w8_thin(const mm_w8_matrix* w, const void* x, int64_t ldx, int32_t M, float* part, int32_t splits,
+                                   int32_t ldp, void* xs_work, void* stream) {
+  return gemm_thin<false>(w, x, ldx, M, part, splits, ldp, xs_work, stream);
+}
+
+extern "C" int32_t mm_gemm_e4m3_thin(const mm_w8_matrix* w, const void* x, int64_t ldx, int32_t M, float* part,
+                                     int32_t splits, int32_t ldp, void* xs_work, void* stream) {
+  return gemm_thin<true>(w, x, ldx, M, part, splits, ldp, xs_work, stream);
+}
+
+extern "C" int32_t mm_quantize_rows_e4m3(const void* x, int64_t ldx, int32_t x_format, int32_t rows, int32_t K,
+                                         const void* gain, uint8_t* q, int64_t ldq, float* scale, void* stream) {
+  MM_REQUIRE(x != nullptr && q != nullptr && scale != nullptr, "mm_quantize_rows_e4m3: null pointer");
+  MM_REQUIRE(rows > 0 && K > 0 && K % 16 == 0 && ldx >= K && ldq >= K && ldq % 16 == 0 && al16(q),
+             "mm_quantize_rows_e4m3: bad shape (rows %d, K %d %% 16, ldx %lld, ldq %lld %% 16, q 16-byte aligned)", rows, K,
+             static_cast<long long>(ldx), static_cast<long long>(ldq));
+  MM_REQUIRE(x_format >= 0 && x_format <= 2, "mm_quantize_rows_e4m3: x_format must be 0 (bf16), 1 (fp16) or 2 (fp32)");
+  MM_REQUIRE(al16(x) && ldx % (x_format == 2 ? 4 : 8) == 0 && (gain == nullptr || al16(gain)),
+             "mm_quantize_rows_e4m3: x and gain must be 16-byte aligned and ldx a whole number of 16-byte units (ldx %lld)",
+             static_cast<long long>(ldx));
+  const bool gf16 = act_f16();
+  auto kern = x_format == 0 ? (gf16 ? quantize_e4m3_kernel<0, true> : quantize_e4m3_kernel<0, false>)
+            : x_format == 1 ? (gf16 ? quantize_e4m3_kernel<1, true> : quantize_e4m3_kernel<1, false>)
+                            : (gf16 ? quantize_e4m3_kernel<2, true> : quantize_e4m3_kernel<2, false>);
+  const cudaError_t e = launch_kernel(kern, dim3(rows), dim3(256), 0, ST(stream), 1, x, static_cast<long long>(ldx), K,
+                                      static_cast<const uint16_t*>(gain), q, static_cast<long long>(ldq), scale);
+  if (e != cudaSuccess) {
+    set_error("mm_quantize_rows_e4m3: launch failed: %s", cudaGetErrorString(e));
+    return 2;
+  }
+  return check_launch("mm_quantize_rows_e4m3");
 }

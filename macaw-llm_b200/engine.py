@@ -638,8 +638,11 @@ class Engine:
         ss_attn = torch.empty((M, E // 32), device=dev, dtype=torch.float32)
         ss_mlp = torch.empty((M, E // 32), device=dev, dtype=torch.float32)
         # int8 decoder (quant.py): decode steps run the int8 GEMM ahead of the same tails; everything else dequantizes one
-        # layer at a time into one scratch buffer and runs the 16-bit GEMMs below unchanged
-        w8 = quant.is_quantized(self.m)
+        # layer at a time into one scratch buffer and runs the 16-bit GEMMs below unchanged.  An FP8 decoder has its own loop.
+        fmt = quant.quant_format(self.m)
+        if fmt == "fp8":
+            return self._llama_layers_fp8(x, B, T, kmask, pos0, cache, dyn, pos_dev, rope, decode, ss_attn, ss_mlp)
+        w8 = fmt == "int8"
         thin = ops.linear_w8_thin_fused if w8 else ops.linear_thin_fused
         if w8 and not decode:
             scratch = torch.empty((3 * E + 2 * I + E) * E + E * I, device=dev, dtype=ADT())
@@ -661,16 +664,7 @@ class Engine:
                 qkv = ops.linear(x, wqkv, epi=ops.EPI_ROPE, rope=rope, **rs_kw)
                 if cache is not None:
                     ops.kv_append(qkv, B, T, cache[i], pos0, pos_dev[0:1] if dyn else None)
-            q5 = qkv.view(B, T, 3, H, hd)
-            if dyn:
-                kv = cache[i].unflatten(-1, (H, hd))  # whole capacity; the kernel reads the valid length from pos_dev[1]
-                a = ops.attention(q5[:, :, 0], kv[:, :, 0], kv[:, :, 1], scale=scale, causal=False, key_mask=kmask,
-                                  tk_dev=pos_dev[1:2])
-            elif pos0 == 0:
-                a = ops.attention(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale=scale, causal=True, key_mask=kmask)
-            else:
-                kv = cache[i][:, : pos0 + T].unflatten(-1, (H, hd))  # (B, Tk, 2, H, hd) view of the cache
-                a = ops.attention(q5[:, :, 0], kv[:, :, 0], kv[:, :, 1], scale=scale, causal=False, key_mask=kmask)
+            a = self._attention(qkv.view(B, T, 3, H, hd), T, i, kmask, pos0, cache, dyn, pos_dev, scale)
             if decode:
                 thin(a.view(B * T, E), wo, ops.THIN_RES, residual=x, out=x, sumsq_out=ss_attn)
                 g = thin(x, wgu, ops.THIN_SWIGLU, rms_from=(ss_attn, eps))
@@ -680,6 +674,49 @@ class Engine:
                 g = ops.linear(x, wgu, epi=ops.EPI_SWIGLU, rms_from=(ss_attn, eps))
                 ops.linear(g, wd, residual=x, out=x, sumsq_out=ss_mlp)
         self._last_ss = None if decode else ss_mlp  # statistics of the final residual stream (consumed by _lm_head)
+        return x
+
+    def _attention(self, q5, T, i, kmask, pos0, cache, dyn, pos_dev, scale):
+        """The decoder's attention over the new rows' q / k / v (prefill) or the KV cache (decode step)."""
+        H, hd = q5.shape[3], q5.shape[4]
+        if dyn:
+            kv = cache[i].unflatten(-1, (H, hd))  # whole capacity; the kernel reads the valid length from pos_dev[1]
+            return ops.attention(q5[:, :, 0], kv[:, :, 0], kv[:, :, 1], scale=scale, causal=False, key_mask=kmask,
+                                 tk_dev=pos_dev[1:2])
+        if pos0 == 0:
+            return ops.attention(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale=scale, causal=True, key_mask=kmask)
+        kv = cache[i][:, : pos0 + T].unflatten(-1, (H, hd))  # (B, Tk, 2, H, hd) view of the cache
+        return ops.attention(q5[:, :, 0], kv[:, :, 0], kv[:, :, 1], scale=scale, causal=False, key_mask=kmask)
+
+    def _llama_layers_fp8(self, x, B, T, kmask, pos0, cache, dyn, pos_dev, rope, decode, ss_attn, ss_mlp):
+        """_llama_layers_impl on an FP8 decoder (quant.quantize_llm_fp8).  Decode steps with up to 64 samples stream the
+        e4m3 weights through mm_gemm_e4m3_thin (activations not quantized) ahead of the 16-bit path's tails.  Everything
+        else quantizes each GEMM input per row (x g1, the attention output, x g2, the SwiGLU output: the RMSNorm gain is
+        applied before quantizing, its row statistic in the epilogue as on the 16-bit path) and runs mm_gemm_e4m3_fwd with
+        the same epilogues."""
+        E, H, hd, I, eps = self._llama_dims()
+        scale = 1.0 / math.sqrt(hd)
+        for i, l in enumerate(self.m.llm.model.layers):
+            wqkv, wgu, wo, wd = self._w8_layer(i, l)
+            rs_kw = dict(row_scale=ops.rms_rstd(x, eps)) if i == 0 else dict(rms_from=(ss_mlp, eps))
+            if decode:
+                thin = ops.linear_w8_thin_fused
+                qkv = thin(x, wqkv, ops.THIN_QKV, rope=(rope[0], rope[1], rope[4] if len(rope) > 4 else None),
+                           cache=cache[i], t0=pos0, t0_dev=pos_dev[0:1] if dyn else None, **rs_kw)
+            else:
+                qkv = ops.linear_e4m3(*ops.quantize_rows_e4m3(x, wqkv.gain), wqkv, epi=ops.EPI_ROPE, rope=rope, **rs_kw)
+                if cache is not None:
+                    ops.kv_append(qkv, B, T, cache[i], pos0, pos_dev[0:1] if dyn else None)
+            a = self._attention(qkv.view(B, T, 3, H, hd), T, i, kmask, pos0, cache, dyn, pos_dev, scale)
+            if decode:
+                thin(a.view(B * T, E), wo, ops.THIN_RES, residual=x, out=x, sumsq_out=ss_attn)
+                g = thin(x, wgu, ops.THIN_SWIGLU, rms_from=(ss_attn, eps))
+                thin(g, wd, ops.THIN_RES, residual=x, out=x, sumsq_out=ss_mlp)
+            else:
+                ops.linear_e4m3(*ops.quantize_rows_e4m3(a.view(B * T, E)), wo, residual=x, out=x, sumsq_out=ss_attn)
+                g = ops.linear_e4m3(*ops.quantize_rows_e4m3(x, wgu.gain), wgu, epi=ops.EPI_SWIGLU, rms_from=(ss_attn, eps))
+                ops.linear_e4m3(*ops.quantize_rows_e4m3(g), wd, residual=x, out=x, sumsq_out=ss_mlp)
+        self._last_ss = None if decode else ss_mlp
         return x
 
     def _lm_head(self, x: torch.Tensor, rows: Optional[torch.Tensor] = None) -> torch.Tensor:

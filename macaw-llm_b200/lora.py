@@ -180,10 +180,12 @@ def add_lora(model, config: LoraConfig) -> Dict[str, nn.Linear]:
         raise TypeError(f"add_lora: expected a LoraConfig, got {type(config).__name__}")
     if adapted_modules(model):
         raise RuntimeError("add_lora: the model already carries adapters (merge_lora() first; one adapter at a time)")
-    from .quant import is_quantized
+    from .quant import quant_format
 
-    if is_quantized(model):
-        raise RuntimeError("add_lora: the decoder is int8-quantized; LoRA needs the 16-bit base weights")
+    fmt = quant_format(model)
+    if fmt is not None:
+        raise RuntimeError(f"add_lora: the decoder is {'int8' if fmt == 'int8' else 'FP8'}-quantized; LoRA needs the 16-bit "
+                           "base weights")
     targets = resolve_targets(model.llm, config)
     from .training import freeze_like_reference
 

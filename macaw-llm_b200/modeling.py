@@ -380,11 +380,15 @@ class MM_LLMs(PreTrainedModel):
         `loss.backward()`): the loss is produced by the kernel-library training step (training.py) and carries a grad_fn
         whose backward runs the hand-written backward pass.  Logits are not returned in this mode (they are consumed in
         place by the cross-entropy backward)."""
-        from .quant import is_quantized
+        from .quant import quant_format
         from .training import TrainStep
 
-        if is_quantized(self):
+        fmt = quant_format(self)
+        if fmt == "int8":
             raise RuntimeError("macaw_b200: the decoder is int8-quantized (quantize_llm_int8) and cannot be trained; call "
+                               "model.eval() / torch.no_grad() for inference")
+        if fmt == "fp8":
+            raise RuntimeError("macaw_b200: the decoder is FP8-quantized (quantize_llm_fp8) and cannot be trained; call "
                                "model.eval() / torch.no_grad() for inference")
         if "_train_step" not in self.__dict__:
             self.__dict__["_train_step"] = TrainStep(self)
@@ -434,6 +438,13 @@ class MM_LLMs(PreTrainedModel):
         from . import quant
 
         quant.quantize_llm_int8(self)
+
+    def quantize_llm_fp8(self) -> None:
+        """Per-row e4m3 weights for the seven projections of every decoder layer, in place; the prefill GEMMs then run on
+        FP8 tensor cores with per-row e4m3 activations.  Inference only; what stays 16-bit is as for quantize_llm_int8."""
+        from . import quant
+
+        quant.quantize_llm_fp8(self)
 
     def prepare_inputs_for_generation(self, inputs):
         return self._engine.prepare_inputs(inputs)

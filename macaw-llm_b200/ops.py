@@ -84,11 +84,13 @@ def gemm_raw(*, M, N, K, A, lda, B, ldb, Cout, ldc, batch=1, a_bs=0, b_bs=0, c_b
              row_scale=None, residual=None, ldr=0, r_bs=0, r_bs2=0, res_row_mod=0, rope_cos=None, rope_sin=None,
              rope_T=0, rope_cols=0, rope_pos=None, c_trans=False, a_fp16=None, b_fp16=None, c_fp16=None,
              bias_rs=None, bias2=None, bias2_rs=None, a_mn_major=False, sumsq_out=None, rs_sumsq=None, rs_parts=0,
-             rs_eps=0.0, streamk=None, plan_only: bool = False):
+             rs_eps=0.0, streamk=None, plan_only: bool = False, e4m3: Optional[_lib.GemmE4m3Args] = None):
     """Direct binding of mm_gemm_fwd; pointers are ints (data_ptr() + byte offsets).  Operand / output formats default to
     the current activation format (ACT()): fp16 for an fp16 model, bf16 otherwise.  `streamk` is a workspace tensor, or
     (address, bytes).  plan_only=True launches nothing and returns the gemm_plan() dict of exactly these arguments
-    (mm_gemm_plan: no memory is touched, so the pointers may be fake); while PLANS is a list, every launch appends its own."""
+    (mm_gemm_plan: no memory is touched, so the pointers may be fake); while PLANS is a list, every launch appends its own.
+    With `e4m3` (mm_gemm_e4m3_args) the call goes to mm_gemm_e4m3_fwd / mm_gemm_e4m3_plan instead: A is the e4m3
+    activation, B is ignored (the weight is e4m3.w)."""
     f16 = ACT() == _F16
     a_fp16 = f16 if a_fp16 is None else a_fp16
     b_fp16 = f16 if b_fp16 is None else b_fp16
@@ -101,16 +103,20 @@ def gemm_raw(*, M, N, K, A, lda, B, ldb, Cout, ldc, batch=1, a_bs=0, b_bs=0, c_b
                  bias_rs, bias2, bias2_rs, int(a_mn_major), sumsq_out, rs_sumsq, int(rs_parts), float(rs_eps),
                  None if streamk is None else streamk[0], 0 if streamk is None else streamk[1])
     if plan_only or PLANS is not None:
-        plan = _plan_of(a)
+        plan = _plan_of(a, e4m3)
         if plan_only:
             return plan
         PLANS.append(plan)
+    if e4m3 is None:
+        fwd, args, what = _lib.load().mm_gemm_fwd, (C.byref(a),), "mm_gemm_fwd"
+    else:
+        fwd, args, what = _lib.load().mm_gemm_e4m3_fwd, (C.byref(a), C.byref(e4m3)), "mm_gemm_e4m3_fwd"
     if PROFILE is None:
-        _check(_lib.load().mm_gemm_fwd(C.byref(a), _stream()), "mm_gemm_fwd")
+        _check(fwd(*args, _stream()), what)
         return
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
-    _check(_lib.load().mm_gemm_fwd(C.byref(a), _stream()), "mm_gemm_fwd")
+    _check(fwd(*args, _stream()), what)
     e1.record()
     PROFILE.append((TAG, 2.0 * M * N * K * batch * max(1, batch2), e0, e1))
 
@@ -141,9 +147,12 @@ def gemm_plan(*, M: int, N: int, K: int, batch: int = 1, batch2: int = 1, epi: i
 PLANS = None
 
 
-def _plan_of(a: GemmArgs) -> dict:
+def _plan_of(a: GemmArgs, e4m3=None) -> dict:
     plan = _lib.GemmPlan()
-    _check(_lib.load().mm_gemm_plan(C.byref(a), C.byref(plan)), "mm_gemm_plan")
+    if e4m3 is None:
+        _check(_lib.load().mm_gemm_plan(C.byref(a), C.byref(plan)), "mm_gemm_plan")
+    else:
+        _check(_lib.load().mm_gemm_e4m3_plan(C.byref(a), C.byref(e4m3), C.byref(plan)), "mm_gemm_e4m3_plan")
     d = {name: int(getattr(plan, name)) for name, _ in _lib.GemmPlan._fields_}
     d["fill"] = d["units"] / float(d["waves"] * d["workers"])  # share of the scheduled tile slots that carry work
     return d
@@ -341,16 +350,20 @@ _W8_CHUNKS = {}  # device copies of the chunk maps, by (rows, interleave, device
 
 
 class W8Matrix:
-    """A fused int8 weight (N, K) over up to three per-row-quantized sources (mm_w8_matrix), the sources' rows arranged
-    as `w8_chunk_map(rows, interleave)` says; `gain` (K,) 16-bit: the RMSNorm gain folded into the product, or None."""
+    """A fused int8 (or e4m3: `fp8`) weight (N, K) over up to three per-row-quantized sources (mm_w8_matrix), the
+    sources' rows arranged as `w8_chunk_map(rows, interleave)` says; `gain` (K,) 16-bit: the RMSNorm gain folded into the
+    product, or None."""
 
     def __init__(self, qs, scales, interleave: bool = False, gain: Optional[torch.Tensor] = None):
         qs, scales = list(qs), list(scales)
         if not 1 <= len(qs) <= _lib.W8_MAX_SRC or len(scales) != len(qs):
             raise ValueError(f"macaw_b200: a fused int8 weight has 1..{_lib.W8_MAX_SRC} sources, each with its scales")
         K = qs[0].shape[1]
+        self.fp8 = qs[0].dtype == _E4M3
         for q, s in zip(qs, scales):
-            if q.dtype != torch.int8 or q.dim() != 2 or not q.is_contiguous() or q.shape[1] != K:
+            if self.fp8 and (q.dtype != _E4M3 or q.dim() != 2 or not q.is_contiguous() or q.shape[1] != K):
+                raise TypeError("macaw_b200: e4m3 sources must be contiguous (rows, K) float8_e4m3fn tensors with one K")
+            if not self.fp8 and (q.dtype != torch.int8 or q.dim() != 2 or not q.is_contiguous() or q.shape[1] != K):
                 raise TypeError("macaw_b200: int8 sources must be contiguous (rows, K) int8 tensors with one K")
             if s.dtype != torch.float32 or tuple(s.shape) != (q.shape[0],) or not s.is_contiguous():
                 raise TypeError("macaw_b200: each source needs a contiguous fp32 scale per row")
@@ -367,7 +380,7 @@ class W8Matrix:
         dchunks = _W8_CHUNKS.get(key)
         if dchunks is None:
             dchunks = _W8_CHUNKS[key] = chunks.to(dev)
-        self.N, self.K = N, K
+        self.N, self.K, self.gain = N, K, gain
         self._keep = (qs, scales, dchunks, gain)
         self.args = _lib.W8Matrix()
         for j, (q, s) in enumerate(zip(qs, scales)):
@@ -395,7 +408,8 @@ def w8_thin_splits(N: int, K: int, n_sms: int) -> int:
 
 def linear_w8_thin_fused(x: torch.Tensor, w: W8Matrix, mode: int, *, splits: Optional[int] = None, **tail) -> torch.Tensor:
     """`linear_thin_fused` on an int8 fused weight: mm_gemm_w8_thin writes the split-K partial sums
-    s_n * sum_k q[n, k] round16(x[m, k] g[k]) and the same mm_thin_fused tail finishes them (keywords as there)."""
+    s_n * sum_k q[n, k] round16(x[m, k] g[k]) and the same mm_thin_fused tail finishes them (keywords as there).  An e4m3
+    weight (w.fp8) runs mm_gemm_e4m3_thin, the same kernel with e4m3(q[n, k])."""
     _cuda(x, ACT(), "x")
     M, K = x.shape
     assert x.stride(1) == 1 and K == w.K and 1 <= M <= 64
@@ -404,9 +418,108 @@ def linear_w8_thin_fused(x: torch.Tensor, w: W8Matrix, mode: int, *, splits: Opt
     Mp = (M + 3) // 4 * 4
     part = torch.empty((S, w.N, Mp), device=dev, dtype=torch.float32)
     xs_work = torch.empty((M, (K + 127) // 128 * 128), device=dev, dtype=ACT())  # x~ when it is streamed
-    _check(_lib.load().mm_gemm_w8_thin(C.byref(w.args), x.data_ptr(), x.stride(0), M, part.data_ptr(), S, Mp,
-                                       xs_work.data_ptr(), _stream()), "mm_gemm_w8_thin")
+    fn, what = (_lib.load().mm_gemm_e4m3_thin, "mm_gemm_e4m3_thin") if w.fp8 else (_lib.load().mm_gemm_w8_thin, "mm_gemm_w8_thin")
+    _check(fn(C.byref(w.args), x.data_ptr(), x.stride(0), M, part.data_ptr(), S, Mp, xs_work.data_ptr(), _stream()), what)
     return _thin_tail(part, M, K, mode, **tail)
+
+
+# ---------------------------------------------------------------------------------------------------- e4m3 (FP8)
+_E4M3 = torch.float8_e4m3fn
+
+
+def quantize_rows_e4m3(x: torch.Tensor, gain: Optional[torch.Tensor] = None):
+    """Per-row e4m3 quantization of a (rows, K) bf16 / fp16 / fp32 matrix (mm_quantize_rows_e4m3) -> (q float8_e4m3fn
+    (rows, K), scale fp32 (rows,)):  v = x g (fp32),  s = max |v| / 448,  q = e4m3(v / s) (nearest even, saturated),
+    q = 0 where s = 0.  `gain` (K,) in the activation format, or None."""
+    if not isinstance(x, torch.Tensor) or x.dim() != 2 or x.dtype not in _W8_FORMAT or x.stride(1) != 1:
+        raise TypeError("macaw_b200: quantize_rows_e4m3 takes a 2-D bf16 / fp16 / fp32 tensor with unit column stride")
+    _cuda(x, None, "x")
+    rows, K = x.shape
+    if gain is not None:
+        _cuda(gain, ACT(), "gain")
+        assert tuple(gain.shape) == (K,) and gain.is_contiguous()
+    q = torch.empty((rows, K), device=x.device, dtype=_E4M3)
+    s = torch.empty((rows,), device=x.device, dtype=torch.float32)
+    args = (x.data_ptr(), x.stride(0), _W8_FORMAT[x.dtype], rows, K, _ptr(gain), q.data_ptr(), K, s.data_ptr(), _stream())
+    if PROFILE is None:
+        _check(_lib.load().mm_quantize_rows_e4m3(*args), "mm_quantize_rows_e4m3")
+        return q, s
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    _check(_lib.load().mm_quantize_rows_e4m3(*args), "mm_quantize_rows_e4m3")
+    e1.record()
+    PROFILE.append((TAG + ".quantize", 0.0, e0, e1))  # no GEMM FLOPs: its time, next to the GEMMs'
+    return q, s
+
+
+def _e4m3_args(a_scale: int, w: W8Matrix, unpromoted: bool) -> _lib.GemmE4m3Args:
+    if not w.fp8:
+        raise TypeError("macaw_b200: the e4m3 GEMM needs an e4m3 weight")
+    e = _lib.GemmE4m3Args()
+    e.a_scale, e.unpromoted = a_scale, int(unpromoted)
+    C.memmove(C.byref(e.w), C.byref(w.args), C.sizeof(_lib.W8Matrix))
+    e.w.gain = None  # the gain was applied to the activation rows before they were quantized
+    return e
+
+
+def linear_e4m3(xq: torch.Tensor, xs: torch.Tensor, w: W8Matrix, *, epi: int = EPI_STD, residual=None,
+                out: Optional[torch.Tensor] = None, out_dtype=None, row_scale: Optional[torch.Tensor] = None, rope=None,
+                sumsq_out: Optional[torch.Tensor] = None, rms_from=None, unpromoted: bool = False,
+                plan_only: bool = False):
+    """`linear` on per-row e4m3 operands: out = epilogue((acc * xs[m]) * s_w[n]), acc = sum_k xq[m, k] q_w[n, k]
+    (mm_gemm_e4m3_fwd).  xq (M, K) float8_e4m3fn with unit column stride and xs (M,) fp32 from quantize_rows_e4m3; w an
+    e4m3 W8Matrix (its gain is not used).  Epilogue keywords as in `linear`; unpromoted=True runs the comparison instance
+    whose MMAs accumulate all of K in place; plan_only=True returns the plan of this launch."""
+    _cuda(xq, _E4M3, "xq"); _cuda(xs, torch.float32, "xs")
+    M, K = xq.shape
+    assert xq.stride(1) == 1 and xs.shape == (M,) and xs.is_contiguous() and K == w.K
+    N = w.N
+    n_out = N // 2 if epi == EPI_SWIGLU else N
+    if out is None:
+        out = torch.empty((M, n_out), device=xq.device, dtype=out_dtype if out_dtype is not None else ACT())
+    assert out.shape == (M, n_out) and out.stride(1) == 1
+    kw = {}
+    if residual is not None:
+        _cuda(residual, ACT(), "residual")
+        assert residual.stride(-1) == 1
+        kw.update(residual=residual.data_ptr(), ldr=residual.stride(0))
+    if rope is not None:
+        cos, sin, T, cols = rope[:4]
+        kw.update(rope_cos=cos.data_ptr(), rope_sin=sin.data_ptr(), rope_T=T, rope_cols=cols)
+        if len(rope) > 4 and rope[4] is not None:
+            kw.update(rope_pos=rope[4].data_ptr())
+    if sumsq_out is not None:
+        assert sumsq_out.dtype == torch.float32 and sumsq_out.is_contiguous() and sumsq_out.shape == (M, (N + 31) // 32)
+        kw.update(sumsq_out=sumsq_out.data_ptr())
+    if rms_from is not None:
+        parts, eps = rms_from
+        assert parts.dtype == torch.float32 and parts.is_contiguous() and parts.shape[0] == M and row_scale is None
+        kw.update(rs_sumsq=parts.data_ptr(), rs_parts=parts.shape[1], rs_eps=eps)
+    e = _e4m3_args(xs.data_ptr(), w, unpromoted)
+    plan = gemm_raw(M=M, N=N, K=K, A=xq.data_ptr(), lda=xq.stride(0), B=0, ldb=K, Cout=out.data_ptr(), ldc=out.stride(0),
+                    c_fp32=out.dtype == torch.float32, c_fp16=out.dtype == _F16, epi=epi, row_scale=_ptr(row_scale),
+                    plan_only=plan_only, e4m3=e, **kw)
+    return plan if plan_only else out
+
+
+def gemm_e4m3_plan(*, M: int, N: int, K: int, epi: int = EPI_STD, rows=None, lda: Optional[int] = None,
+                   a_scale: bool = True, w_scale: bool = True) -> dict:
+    """The launch mm_gemm_e4m3_fwd would make for M activation rows against an e4m3 weight (N, K) whose sources have
+    `rows` (default one source of N rows), 16-byte-aligned fake operands (mm_gemm_e4m3_plan: nothing is touched, no GPU
+    needed).  a_scale / w_scale=False pass null scales (argument checks)."""
+    lib = _lib.load()
+    fake = 1 << 20
+    rows = [N] if rows is None else list(rows)
+    n_out = N // 2 if epi == EPI_SWIGLU else N
+    rope = dict(rope_cos=fake, rope_sin=fake, rope_T=max(1, M), rope_cols=(N // 128) * 128) if epi == EPI_ROPE else {}
+    a = GemmArgs(M=M, N=N, K=K, batch=1, batch2=1, A=fake, lda=K if lda is None else lda, B=fake, ldb=K, C=fake,
+                 ldc=n_out, epi=epi, alpha=1.0, c_fp16=int(ACT() == _F16), **rope)
+    e = _lib.GemmE4m3Args()
+    e.a_scale = fake if a_scale else None
+    for j, r in enumerate(rows):
+        e.w.q[j], e.w.scale[j], e.w.rows[j] = fake, fake if w_scale else None, r
+    e.w.chunks, e.w.N, e.w.K = fake, N, K
+    return _plan_of(a, e)
 
 
 def splitk_reduce(partial: torch.Tensor, bias: Optional[torch.Tensor], out: torch.Tensor) -> torch.Tensor:

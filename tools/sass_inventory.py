@@ -2,7 +2,7 @@
 """SASS / resource inventory of libmacaw_b200.so (no GPU needed: `cuobjdump` reads the cubin nvcc cross-compiled).
 
 Per kernel: registers, static + dynamic-independent shared memory, local (spill) bytes, and how often the Hopper
-mnemonics that prove a wgmma / TMA / mbarrier kernel appear (HGMMA = wgmma.mma_async, UTMALDG = TMA tensor load,
+mnemonics that prove a wgmma / TMA / mbarrier kernel appear (HGMMA = wgmma.mma_async: HGMMA on 16-bit, QGMMA on e4m3 operands, UTMALDG = TMA tensor load,
 SYNCS = mbarrier operations, WARPGROUP = warpgroup arrive / wait) next to HMMA (mma.sync).
 Usage: python tools/sass_inventory.py
 """
@@ -16,7 +16,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "macaw-llm_b200", "libmacaw_b200.so")
 
 COLS = OrderedDict([
-    ("HGMMA", r"\bHGMMA\."), ("UTMALDG", r"\bUTMALDG"), ("SYNCS", r"\bSYNCS\."), ("WARPGROUP", r"\bWARPGROUP\."),
+    ("HGMMA", r"\b[HQ]GMMA\."), ("UTMALDG", r"\bUTMALDG"), ("SYNCS", r"\bSYNCS\."), ("WARPGROUP", r"\bWARPGROUP\."),
     ("HMMA", r"\bHMMA\."), ("MUFU.EX2", r"\bMUFU\.EX2"),
 ])
 
@@ -29,7 +29,7 @@ def demangle(names):
     out = run("c++filt", *names).splitlines()
     short = []
     for n in out:
-        n = re.sub(r"^void ", "", n)
+        n = re.sub(r"^void ", "", n).replace("(anonymous namespace)::", "")
         n = re.sub(r"\(.*$", "", n)  # drop the parameter list
         short.append(n.replace("mm::", ""))
     return dict(zip(names, short))
@@ -68,7 +68,7 @@ def main():
     arch = re.search(r"arch = (\S+)", run("cuobjdump", "-lelf", LIB) + sass)
     print(f"# tools/sass_inventory.py over macaw-llm_b200/libmacaw_b200.so ({arch.group(1) if arch else '?'}; "
           f"{len(counts)} kernels; cuobjdump -sass / --dump-resource-usage, no GPU involved)")
-    print("# HGMMA = wgmma.mma_async, UTMALDG = TMA tensor load, SYNCS = mbarrier operations, WARPGROUP = warpgroup")
+    print("# HGMMA = wgmma.mma_async (HGMMA / QGMMA), UTMALDG = TMA tensor load, SYNCS = mbarrier operations, WARPGROUP = warpgroup")
     print("# arrive / wait, HMMA = mma.sync, LOCAL = spill bytes")
     hdr = f"{'kernel':64s} {'REG':>4s} {'SMEM':>6s} {'LOCAL':>5s} " + " ".join(f"{k:>12s}" for k in COLS)
     print(hdr)
