@@ -282,6 +282,27 @@ int64_t mm_align_workspace_bytes(int32_t R, int32_t V);
 int32_t mm_kv_append(const void* qkv, int64_t ld_qkv, int32_t B, int32_t T_new, int32_t E, void* cache, int32_t Tmax,
                      int32_t t0, const int32_t* t0_dev, void* stream); /* t0_dev != NULL overrides t0 with a device int */
 int32_t mm_argmax_rows(const void* logits, int64_t ld, int32_t rows, int32_t V, int64_t* out, void* stream);
+/* The int8 KV cache of the generate branch (same reference KV-cache logic, modeling.py:190-195, with K / V stored in int8).
+ * Each cached key vector and each cached value vector of one token and one head (hd = 128 elements) is quantized on its
+ * own.  v is the vector as the 16-bit cache would store it (keys after RoPE, rounded to the activation format):
+ *   s = fp32(max_d |v_d|) / 127 (IEEE division),  q_d = clamp(rint(v_d / s), -127, 127) (IEEE division, ties to even),
+ *   q = 0 where s = 0;  the dequantized value is the fp32 product q_d * s.
+ * Layout per layer: cache int8 (B, Tmax, 2, E), indexed as the 16-bit cache; cache_scale fp32 (B, 2, H, Tmax), so one head's
+ * scales run contiguously along the key axis.
+ * mm_kv_append_i8: mm_kv_append's copy with that quantization (same arguments plus cache_scale; t0_dev overrides t0). */
+int32_t mm_kv_append_i8(const void* qkv, int64_t ld_qkv, int32_t B, int32_t T_new, int32_t E, int8_t* cache,
+                        float* cache_scale, int32_t Tmax, int32_t t0, const int32_t* t0_dev, void* stream);
+/* mm_attn_decode_i8: one query row per (b, h) over the int8 cache (the decode step's attention, no mask):
+ * out[b, h] = softmax_t(scale * s_k[t] * sum_d q_d kq[t, d]) . (s_v[t] vq[t]) over keys t < Tk, with Tk = min(*tk_dev, Tk)
+ * when tk_dev is given (so a captured graph reads the count).  q 16-bit, element (b, h, d) at q[b * q_bs + h * 128 + d];
+ * out likewise with o_bs.  Keys at or past the count are never read (neither values nor scales).  The keys are split over
+ * CTAs by a layout that depends only on (B, H, Tmax, SM count); each split keeps its running max, sum and output in fp32 and
+ * a second kernel merges the splits in a fixed order, so results are deterministic.  workspace: fp32, at least
+ * mm_attn_decode_i8_workspace_bytes(B, H, Tmax) bytes.  No key: zeros. */
+int32_t mm_attn_decode_i8(const void* q, int64_t q_bs, const int8_t* cache, const float* cache_scale, void* out,
+                          int64_t o_bs, int32_t B, int32_t H, int32_t Tmax, int32_t Tk, const int32_t* tk_dev, float scale,
+                          float* workspace, int64_t workspace_bytes, void* stream);
+int64_t mm_attn_decode_i8_workspace_bytes(int32_t B, int32_t H, int32_t Tmax);
 /* mm_sample_rows: the next token of HF generate's decoding step (reference modeling.py:959 -> llm.generate with
  * llm.generation_config): RepetitionPenaltyLogitsProcessor -> TemperatureLogitsWarper -> TopKLogitsWarper ->
  * TopPLogitsWarper -> softmax -> multinomial, in fp32 on the 16-bit logits (rows, V), row stride ld, V <= 49152.
@@ -328,6 +349,11 @@ typedef struct mm_thin_args {
   const int32_t* t0_dev;
 } mm_thin_args;
 int32_t mm_thin_fused(const mm_thin_args* args, void* stream);
+/* mm_thin_fused_kv_i8: the MM_THIN_QKV tail with an int8 cache (see mm_kv_append_i8).  k / v are rounded to 16 bits as
+ * MM_THIN_QKV stores them, then each head vector is quantized into args->cache (int8 (B, Tmax, 2, E)) and cache_scale
+ * (fp32 (B, 2, H, Tmax)) at slot t0 (*t0_dev if given); q rows -> out in 16 bits as in MM_THIN_QKV.  args->mode must be
+ * MM_THIN_QKV. */
+int32_t mm_thin_fused_kv_i8(const mm_thin_args* args, float* cache_scale, void* stream);
 /* In-place rotate-half RoPE (head_dim 128, apply_rotary_pos_emb modeling.py:83-91) on the first rot_cols columns of each
  * row; position of row r = (*pos_dev if given) + r % rope_T.  The training step's RoPE backward calls it with the sin
  * table negated (the rotation is orthogonal: its transpose is the rotation by -theta). */

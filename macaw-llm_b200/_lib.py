@@ -188,10 +188,15 @@ SIGNATURES = {
     "mm_align_fwd": (c_i32, [C.POINTER(AlignArgs), c_vp]),
     "mm_align_workspace_bytes": (c_i64, [c_i32, c_i32]),
     "mm_kv_append": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_i32, c_vp, c_i32, c_i32, c_vp, c_vp]),
+    "mm_kv_append_i8": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_i32, c_vp, c_vp, c_i32, c_i32, c_vp, c_vp]),
+    "mm_attn_decode_i8": (c_i32, [c_vp, c_i64, c_vp, c_vp, c_vp, c_i64, c_i32, c_i32, c_i32, c_i32, c_vp, c_f32, c_vp, c_i64,
+                                  c_vp]),
+    "mm_attn_decode_i8_workspace_bytes": (c_i64, [c_i32, c_i32, c_i32]),
     "mm_gemm_streamk_workspace_bytes": (c_i64, []),
     "mm_gemm_streamk_mode": (c_i32, [c_i32]),
     "mm_gemm_overlap_mode": (c_i32, [c_i32]),
     "mm_thin_fused": (c_i32, [C.POINTER(ThinArgs), c_vp]),
+    "mm_thin_fused_kv_i8": (c_i32, [C.POINTER(ThinArgs), c_vp, c_vp]),
     "mm_argmax_rows": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_vp]),
     "mm_sample_rows": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_f32, c_f32, c_i32, c_f32, c_i32, c_vp, c_vp, c_vp, c_vp]),
     "mm_rope_rows": (c_i32, [c_vp, c_i64, c_i32, c_i32, c_vp, c_vp, c_i32, c_vp, c_vp]),

@@ -364,6 +364,9 @@ __global__ void rope_rows_kernel(bf16* __restrict__ x, long long ld, int rows, i
 //   MM_THIN_QKV    rotate-half RoPE (head_dim 128, pairs (i, i + 64)) on the q and k features in fp32 — exactly what the
 //                  prefill GEMM's RoPE epilogue does —, q -> out[m][n], k / v -> straight into the layer's KV cache slot
 //                  (B, Tmax, 2, E) at position t0 (row m = sample m: one new token per sample)
+//   kThinQkvI8     the same with an int8 cache (mm_thin_fused_kv_i8): each k / v head vector is rounded to 16 bits as
+//                  MM_THIN_QKV stores it, then quantized by the int8 KV-cache rule (kv_quant_scale / kv_quant, ptx.cuh)
+//                  into cache + cache_scale
 // rs_m = row_scale[m], or rsqrt(sum_j rs_sumsq[m][j] / rs_K + rs_eps) from the statistics a MM_THIN_RES pass left (fixed
 // summation order: deterministic), or 1.
 struct ThinFusedParams {
@@ -382,13 +385,17 @@ struct ThinFusedParams {
   const float* rope_sin;
   const int* pos_dev;
   int E;
-  bf16* cache;
+  void* cache;  // 16-bit (MM_THIN_QKV) or int8 (kThinQkvI8)
   int Tmax, t0;
   const int* t0_dev;
+  float* cache_scale;  // kThinQkvI8: (B, 2, H, Tmax) fp32
 };
+constexpr int kThinQkvI8 = 3;  // the kernel's mode for mm_thin_fused_kv_i8 (not an mm_thin_args mode)
 
 template <bool F16, int MODE>
 __global__ void __launch_bounds__(64) thin_fused_kernel(const ThinFusedParams p) {
+  constexpr bool kQKV = MODE == MM_THIN_QKV || MODE == kThinQkvI8;
+  __shared__ float head_max[2][2][8];  // kThinQkvI8: [m0 pass parity][warp][row] of the k / v head's |max|
   griddep_launch();
   griddep_wait();
   const int lane = threadIdx.x & 31;
@@ -410,7 +417,7 @@ __global__ void __launch_bounds__(64) thin_fused_kernel(const ThinFusedParams p)
   // is issued before the first dependent instruction (fully unrolled, predicated), and the one dependent pair (RoPE table
   // row <- device-side position) comes last: two L2 round trips in total instead of one per loop iteration.
   int pos = 0, t0 = p.t0;
-  if (MODE == MM_THIN_QKV) {  // one new token per sample: every row shares the position and the cache slot
+  if (kQKV) {  // one new token per sample: every row shares the position and the cache slot
     if (p.pos_dev != nullptr) pos = *p.pos_dev;
     if (p.t0_dev != nullptr) t0 = *p.t0_dev;
   }
@@ -454,7 +461,7 @@ __global__ void __launch_bounds__(64) thin_fused_kernel(const ThinFusedParams p)
       for (int j = 0; j < 8; ++j)
         if (m0 + j < p.M) resv[j] = ldv<F16>(p.residual[static_cast<long long>(m0 + j) * p.ldr + n1]);
     }
-    if (MODE == MM_THIN_QKV && m0 == 0) {  // depends on `pos`: issued after everything else is in flight
+    if (kQKV && m0 == 0) {  // depends on `pos`: issued after everything else is in flight
       const int jj = (unit & 1) * 32 + lane;
       rope_c = p.rope_cos[static_cast<long long>(pos) * 64 + jj];
       rope_s = p.rope_sin[static_cast<long long>(pos) * 64 + jj];
@@ -521,12 +528,47 @@ __global__ void __launch_bounds__(64) thin_fused_kernel(const ThinFusedParams p)
         if (n1 < p.E) {
           p.out[static_cast<long long>(m) * p.ldo + n1] = stv<F16>(x1);
           p.out[static_cast<long long>(m) * p.ldo + n2] = stv<F16>(x2);
-        } else {
+        } else if (MODE == MM_THIN_QKV) {
           const int which = n1 < 2 * p.E ? 0 : 1;
-          bf16* dst = p.cache + ((static_cast<long long>(m) * p.Tmax + t0) * 2 + which) * p.E + (n1 - (which + 1) * p.E);
+          bf16* dst = static_cast<bf16*>(p.cache) + ((static_cast<long long>(m) * p.Tmax + t0) * 2 + which) * p.E +
+                      (n1 - (which + 1) * p.E);
           dst[0] = stv<F16>(x1);
           dst[64] = stv<F16>(x2);
+        } else {  // the 16-bit values the 16-bit cache would hold, kept for the head's quantization below
+          a1[j] = ldv<F16>(stv<F16>(x1));
+          a2[j] = ldv<F16>(stv<F16>(x2));
         }
+      }
+    }
+    if (MODE == kThinQkvI8 && n1 >= p.E) {  // block-uniform: both warps hold halves of the same k / v head
+      // |max| over the head: each warp's half by shuffles, the two halves through shared memory (one barrier per pass;
+      // the parity buffer keeps a fast warp's next pass off the slots the other warp may still read)
+      const int par = (m0 >> 3) & 1, warp = threadIdx.x >> 5;
+      float mx[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) mx[j] = m0 + j < p.M ? fmaxf(fabsf(a1[j]), fabsf(a2[j])) : 0.f;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) mx[j] = fmaxf(mx[j], __shfl_xor_sync(0xffffffffu, mx[j], o));
+      }
+      if (lane == 0) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) head_max[par][warp][j] = mx[j];
+      }
+      __syncthreads();
+      const int which = n1 < 2 * p.E ? 0 : 1;
+      const int col = n1 - (which + 1) * p.E, head = col >> 7;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int m = m0 + j;
+        if (m >= p.M) break;  // block-uniform
+        const float s = kv_quant_scale(fmaxf(head_max[par][0][j], head_max[par][1][j]));
+        int8_t* dst = static_cast<int8_t*>(p.cache) + ((static_cast<long long>(m) * p.Tmax + t0) * 2 + which) * p.E + col;
+        dst[0] = kv_quant(a1[j], s);
+        dst[64] = kv_quant(a2[j], s);
+        if (threadIdx.x == 0)
+          p.cache_scale[((static_cast<long long>(m) * 2 + which) * (p.E >> 7) + head) * p.Tmax + t0] = s;
       }
     }
   }
@@ -972,7 +1014,8 @@ extern "C" int32_t mm_rope_rows(void* x, int64_t ld, int32_t rows, int32_t rot_c
   return check_launch("mm_rope_rows");
 }
 
-extern "C" int32_t mm_thin_fused(const mm_thin_args* a, void* stream) {
+// mm_thin_fused, or with cache_scale its int8-cache QKV form mm_thin_fused_kv_i8
+static int32_t thin_fused(const mm_thin_args* a, float* cache_scale, void* stream) {
   MM_REQUIRE(a != nullptr && a->part && a->out && a->splits > 0 && a->N > 0 && a->M > 0 && a->ldp >= a->M,
              "mm_thin_fused: bad arguments");
   MM_REQUIRE(a->mode >= MM_THIN_RES && a->mode <= MM_THIN_QKV, "mm_thin_fused: bad mode %d", a->mode);
@@ -989,7 +1032,7 @@ extern "C" int32_t mm_thin_fused(const mm_thin_args* a, void* stream) {
   p.row_scale = a->row_scale; p.rs_sumsq = a->rs_sumsq; p.rs_parts = a->rs_parts; p.rs_K = a->rs_K; p.rs_eps = a->rs_eps;
   p.residual = (const bf16*)a->residual; p.ldr = a->ldr; p.out = (bf16*)a->out; p.ldo = a->ldo; p.sumsq_out = a->sumsq_out;
   p.rope_cos = a->rope_cos; p.rope_sin = a->rope_sin; p.pos_dev = a->pos_dev; p.E = a->E;
-  p.cache = (bf16*)a->cache; p.Tmax = a->Tmax; p.t0 = a->t0; p.t0_dev = a->t0_dev;
+  p.cache = a->cache; p.Tmax = a->Tmax; p.t0 = a->t0; p.t0_dev = a->t0_dev; p.cache_scale = cache_scale;
   const int units = a->mode == MM_THIN_RES ? a->N / 32 : a->N / 64;
   const dim3 grid((units + 1) / 2), block(64);
   const bool f16 = act_f16();
@@ -999,13 +1042,22 @@ extern "C" int32_t mm_thin_fused(const mm_thin_args* a, void* stream) {
           : launch_kernel(thin_fused_kernel<false, MODE_>, grid, block, 0, ST(stream), 1, p)
   if (a->mode == MM_THIN_RES) MM_TF(MM_THIN_RES);
   else if (a->mode == MM_THIN_SWIGLU) MM_TF(MM_THIN_SWIGLU);
-  else MM_TF(MM_THIN_QKV);
+  else if (cache_scale == nullptr) MM_TF(MM_THIN_QKV);
+  else MM_TF(kThinQkvI8);
 #undef MM_TF
   if (e != cudaSuccess) {
     set_error("mm_thin_fused: launch failed: %s", cudaGetErrorString(e));
     return 2;
   }
   return check_launch("mm_thin_fused");
+}
+
+extern "C" int32_t mm_thin_fused(const mm_thin_args* a, void* stream) { return thin_fused(a, nullptr, stream); }
+
+extern "C" int32_t mm_thin_fused_kv_i8(const mm_thin_args* a, float* cache_scale, void* stream) {
+  MM_REQUIRE(a != nullptr && a->mode == MM_THIN_QKV && cache_scale != nullptr,
+             "mm_thin_fused_kv_i8: needs mode MM_THIN_QKV and the cache_scale buffer");
+  return thin_fused(a, cache_scale, stream);
 }
 
 extern "C" int32_t mm_argmax_rows(const void* logits, int64_t ld, int32_t rows, int32_t V, int64_t* out, void* stream) {

@@ -365,4 +365,11 @@ __device__ __forceinline__ float ldv(__nv_bfloat16 v) { return cvt_in<F16>(__bfl
 template <bool F16>
 __device__ __forceinline__ __nv_bfloat16 stv(float v) { return __ushort_as_bfloat16(cvt_out<F16>(v)); }
 
+// The int8 KV-cache rule (include/macaw_b200.h, mm_kv_append_i8): the per-row rule of mm_quantize_rows_int8 applied to one
+// 128-element head vector v:  s = fp32(max |v|) / 127,  q = clamp(rint(v / s), -127, 127),  q = 0 where s = 0.
+__device__ __forceinline__ float kv_quant_scale(float absmax) { return __fdiv_rn(absmax, 127.0f); }
+__device__ __forceinline__ int8_t kv_quant(float v, float s) {
+  return s != 0.f ? static_cast<int8_t>(max(-127, min(127, __float2int_rn(__fdiv_rn(v, s))))) : static_cast<int8_t>(0);
+}
+
 }  // namespace mm

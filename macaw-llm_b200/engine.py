@@ -31,6 +31,65 @@ def _round_up(x: int, m: int) -> int:
     return (x + m - 1) // m * m
 
 
+class KVCache:
+    """The generate branch's per-layer K / V cache, 16-bit: one (B, t_max, 2, E) tensor per layer in the activation format.
+
+    The cache format is decided here and nowhere else: the decoder loop asks its cache to append the prefill's (or a wide
+    decode step's) k / v rows, for the decode tail's keywords, and for a decode step's attention over it."""
+
+    def __init__(self, layers):
+        self.layers = layers
+
+    @classmethod
+    def allocate(cls, B: int, t_max: int, n_layers: int, E: int, dev) -> "KVCache":
+        return cls([torch.zeros((B, t_max, 2, E), device=dev, dtype=ADT()) for _ in range(n_layers)])
+
+    def append(self, i: int, qkv: torch.Tensor, B: int, T: int, pos0: int, t0_dev: Optional[torch.Tensor]) -> None:
+        ops.kv_append(qkv, B, T, self.layers[i], pos0, t0_dev)
+
+    def tail_kw(self, i: int) -> dict:
+        """Keywords of the THIN_QKV decode tail that writes this layer's slot."""
+        return dict(cache=self.layers[i])
+
+    def attend(self, i: int, q: torch.Tensor, T: int, kmask, pos0: int, pos_dev: Optional[torch.Tensor], scale: float):
+        """A decode step's attention of q (B, T, H, hd) over keys [0, pos0 + T), or [0, pos_dev[1]) when pos_dev is given
+        (the whole capacity is handed over; the kernel reads the valid length)."""
+        H, hd = q.shape[2], q.shape[3]
+        if pos_dev is not None:
+            kv = self.layers[i].unflatten(-1, (H, hd))
+            return ops.attention(q, kv[:, :, 0], kv[:, :, 1], scale=scale, causal=False, key_mask=kmask, tk_dev=pos_dev[1:2])
+        kv = self.layers[i][:, : pos0 + T].unflatten(-1, (H, hd))  # (B, Tk, 2, H, hd) view of the cache
+        return ops.attention(q, kv[:, :, 0], kv[:, :, 1], scale=scale, causal=False, key_mask=kmask)
+
+
+class KVCacheInt8(KVCache):
+    """The int8 KV cache (Engine.enable_int8_kv_cache): per layer, int8 values `kq` (B, t_max, 2, E), indexed as the 16-bit
+    cache, and fp32 scales `ks` (B, 2, H, t_max), one per (token, head) key or value vector of 128 elements:
+    s = fp32(max |v|) / 127, q = clamp(rint(v / s), -127, 127), q = 0 where s = 0, for v as the 16-bit cache would hold it.
+    A decode step's attention runs mm_attn_decode_i8 on the dequantized q * s."""
+
+    def __init__(self, kq, ks):
+        super().__init__(kq)
+        self.ks = ks
+
+    @classmethod
+    def allocate(cls, B: int, t_max: int, n_layers: int, E: int, dev) -> "KVCacheInt8":
+        return cls([torch.zeros((B, t_max, 2, E), device=dev, dtype=torch.int8) for _ in range(n_layers)],
+                   [torch.zeros((B, 2, E // 128, t_max), device=dev, dtype=torch.float32) for _ in range(n_layers)])
+
+    def append(self, i, qkv, B, T, pos0, t0_dev):
+        ops.kv_append_i8(qkv, B, T, self.layers[i], self.ks[i], pos0, t0_dev)
+
+    def tail_kw(self, i):
+        return dict(cache=self.layers[i], cache_scale=self.ks[i])
+
+    def attend(self, i, q, T, kmask, pos0, pos_dev, scale):
+        assert T == 1
+        if pos_dev is not None:
+            return ops.attention_decode_i8(q, self.layers[i], self.ks[i], scale=scale, tk_dev=pos_dev[1:2], key_mask=kmask)
+        return ops.attention_decode_i8(q, self.layers[i], self.ks[i], scale=scale, Tk=pos0 + T, key_mask=kmask)
+
+
 class Engine:
     def __init__(self, model):
         self.m = model
@@ -50,6 +109,7 @@ class Engine:
         self.streamk = True
         self._sk_ws: Dict[str, torch.Tensor] = {}
         self._graphs_on = False
+        self.kv_int8 = False  # generate keeps its KV cache in int8 (enable_int8_kv_cache)
         self.align_max_rows = None  # test hook: cap on query rows per alignment chunk (default: ~2 GiB of fp32 scores)
 
     # ------------------------------------------------------------------------------------------------ weight cache
@@ -611,8 +671,9 @@ class Engine:
         """The decoder stack on the residual stream x (B*T, E), updated in place.
 
         pos0 = position of the first row of every sample (0 for prefill, the current length for a decode step).
-        With `cache` (per layer (B, Tmax, 2, E)) the new K/V rows are appended at pos0 and, for decode steps (pos0 > 0),
-        attention reads keys/values [0, pos0 + T) from the cache (reference KV-cache logic: modeling.py:190-195).
+        With `cache` (a KVCache, or a list of per-layer (B, Tmax, 2, E) 16-bit tensors) the new K/V rows are appended at
+        pos0 and, for decode steps (pos0 > 0), attention reads keys/values [0, pos0 + T) from the cache (reference KV-cache
+        logic: modeling.py:190-195).
         `pos_dev` (int32 tensor [pos, pos + 1] on the device) replaces pos0 for a decode step whose launches are captured
         in a CUDA graph: RoPE position, cache slot and key count are then read by the kernels themselves."""
         E, H, hd, I, eps = self._llama_dims()
@@ -634,6 +695,8 @@ class Engine:
         # gate-up / lm_head) derives rsqrt(mean(x^2) + eps) from them — no separate pass over the stream after the first
         # layer's input.
         M = x.shape[0]
+        if cache is not None and not isinstance(cache, KVCache):
+            cache = KVCache(cache)
         decode = cache is not None and T == 1 and B <= 64
         ss_attn = torch.empty((M, E // 32), device=dev, dtype=torch.float32)
         ss_mlp = torch.empty((M, E // 32), device=dev, dtype=torch.float32)
@@ -659,11 +722,11 @@ class Engine:
             rs_kw = dict(row_scale=ops.rms_rstd(x, eps)) if i == 0 else dict(rms_from=(ss_mlp, eps))
             if decode:
                 qkv = thin(x, wqkv, ops.THIN_QKV, rope=(rope[0], rope[1], rope[4] if len(rope) > 4 else None),
-                           cache=cache[i], t0=pos0, t0_dev=pos_dev[0:1] if dyn else None, **rs_kw)
+                           t0=pos0, t0_dev=pos_dev[0:1] if dyn else None, **cache.tail_kw(i), **rs_kw)
             else:
                 qkv = ops.linear(x, wqkv, epi=ops.EPI_ROPE, rope=rope, **rs_kw)
                 if cache is not None:
-                    ops.kv_append(qkv, B, T, cache[i], pos0, pos_dev[0:1] if dyn else None)
+                    cache.append(i, qkv, B, T, pos0, pos_dev[0:1] if dyn else None)
             a = self._attention(qkv.view(B, T, 3, H, hd), T, i, kmask, pos0, cache, dyn, pos_dev, scale)
             if decode:
                 thin(a.view(B * T, E), wo, ops.THIN_RES, residual=x, out=x, sumsq_out=ss_attn)
@@ -678,15 +741,9 @@ class Engine:
 
     def _attention(self, q5, T, i, kmask, pos0, cache, dyn, pos_dev, scale):
         """The decoder's attention over the new rows' q / k / v (prefill) or the KV cache (decode step)."""
-        H, hd = q5.shape[3], q5.shape[4]
-        if dyn:
-            kv = cache[i].unflatten(-1, (H, hd))  # whole capacity; the kernel reads the valid length from pos_dev[1]
-            return ops.attention(q5[:, :, 0], kv[:, :, 0], kv[:, :, 1], scale=scale, causal=False, key_mask=kmask,
-                                 tk_dev=pos_dev[1:2])
-        if pos0 == 0:
+        if pos0 == 0 and not dyn:
             return ops.attention(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], scale=scale, causal=True, key_mask=kmask)
-        kv = cache[i][:, : pos0 + T].unflatten(-1, (H, hd))  # (B, Tk, 2, H, hd) view of the cache
-        return ops.attention(q5[:, :, 0], kv[:, :, 0], kv[:, :, 1], scale=scale, causal=False, key_mask=kmask)
+        return cache.attend(i, q5[:, :, 0], T, kmask, pos0, pos_dev if dyn else None, scale)
 
     def _llama_layers_fp8(self, x, B, T, kmask, pos0, cache, dyn, pos_dev, rope, decode, ss_attn, ss_mlp):
         """_llama_layers_impl on an FP8 decoder (quant.quantize_llm_fp8).  Decode steps with up to 64 samples stream the
@@ -702,11 +759,11 @@ class Engine:
             if decode:
                 thin = ops.linear_w8_thin_fused
                 qkv = thin(x, wqkv, ops.THIN_QKV, rope=(rope[0], rope[1], rope[4] if len(rope) > 4 else None),
-                           cache=cache[i], t0=pos0, t0_dev=pos_dev[0:1] if dyn else None, **rs_kw)
+                           t0=pos0, t0_dev=pos_dev[0:1] if dyn else None, **cache.tail_kw(i), **rs_kw)
             else:
                 qkv = ops.linear_e4m3(*ops.quantize_rows_e4m3(x, wqkv.gain), wqkv, epi=ops.EPI_ROPE, rope=rope, **rs_kw)
                 if cache is not None:
-                    ops.kv_append(qkv, B, T, cache[i], pos0, pos_dev[0:1] if dyn else None)
+                    cache.append(i, qkv, B, T, pos0, pos_dev[0:1] if dyn else None)
             a = self._attention(qkv.view(B, T, 3, H, hd), T, i, kmask, pos0, cache, dyn, pos_dev, scale)
             if decode:
                 thin(a.view(B * T, E), wo, ops.THIN_RES, residual=x, out=x, sumsq_out=ss_attn)
@@ -799,11 +856,12 @@ class Engine:
             # device-side key count, so the caches are not re-zeroed.
             t_max = _round_up(T + max_new_tokens, 64)
             stamp = self._stamp(*self.m.llm.parameters())
-            key = (B, t_max, str(dev))
+            kv_cls = KVCacheInt8 if self.kv_int8 else KVCache
+            key = (B, t_max, str(dev), kv_cls.__name__)
             st = self._decode.get(key)
             if st is None or st["stamp"] != stamp:
                 st = dict(stamp=stamp, graphs={},
-                          cache=[torch.zeros((B, t_max, 2, E), device=dev, dtype=ADT()) for _ in range(n_layers)],
+                          cache=kv_cls.allocate(B, t_max, n_layers, E, dev),
                           finished=torch.zeros((B,), device=dev, dtype=torch.bool),
                           pos_dev=torch.zeros((2,), device=dev, dtype=torch.int32),
                           tok_in=torch.zeros((B,), device=dev, dtype=torch.int64))
@@ -910,6 +968,14 @@ class Engine:
         self._graphs_on = bool(flag)
         if not flag:
             self._graphs.clear()
+
+    def enable_int8_kv_cache(self, flag: bool = True) -> None:
+        """Keep generate()'s KV cache in int8 (KVCacheInt8: one fp32 scale per token and head for keys and for values),
+        about half the bytes of the 16-bit cache.  The prefill's attention still reads its fresh 16-bit q / k / v, so the
+        first generated token is the 16-bit cache's; decode steps attend over the dequantized cache.  The decode state
+        is dropped, so the other format's buffers are freed.  The eval forward and the training step are unaffected."""
+        self.kv_int8 = bool(flag)
+        self._decode.clear()
 
     _TENSOR_KEYS = ("images", "audios", "videos", "input_ids", "attention_mask", "labels", "image_starts", "image_ends",
                     "audio_starts", "audio_ends", "video_starts", "video_ends")

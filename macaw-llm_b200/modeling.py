@@ -446,6 +446,11 @@ class MM_LLMs(PreTrainedModel):
 
         quant.quantize_llm_fp8(self)
 
+    def enable_int8_kv_cache(self, flag: bool = True) -> None:
+        """Generate with an int8 KV cache (per-(token, head) fp32 scales; Engine.enable_int8_kv_cache), or with the
+        16-bit cache again (flag=False).  Affects `inputs['inference'] = True` only; off by default."""
+        self._engine.enable_int8_kv_cache(flag)
+
     def prepare_inputs_for_generation(self, inputs):
         return self._engine.prepare_inputs(inputs)
 

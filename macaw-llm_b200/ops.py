@@ -249,13 +249,15 @@ THIN_RES, THIN_SWIGLU, THIN_QKV = 0, 1, 2
 def linear_thin_fused(x: torch.Tensor, w: torch.Tensor, mode: int, *, row_scale: Optional[torch.Tensor] = None,
                       rms_from=None, residual: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
                       sumsq_out: Optional[torch.Tensor] = None, rope=None, cache: Optional[torch.Tensor] = None, t0: int = 0,
-                      t0_dev: Optional[torch.Tensor] = None, splits: Optional[int] = None) -> torch.Tensor:
+                      t0_dev: Optional[torch.Tensor] = None, splits: Optional[int] = None,
+                      cache_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Decode-step GEMM x (M <= 64, K) @ w (N, K)^T with K split over `splits` CTAs per weight tile (fp32 partials) and ONE
     fused tail kernel (mm_thin_fused):
       THIN_RES     out = rs * xW^T + residual (in place allowed); sumsq_out (M, N/32) fp32 receives the next RMSNorm's statistic
       THIN_SWIGLU  out (M, N/2) = silu(gate) * up of the [32 gate | 32 up]-interleaved fused weight
       THIN_QKV     N = 3E: RoPE on q / k (rope = (cos, sin, pos_dev | None)), q -> out (M, 3E) columns [0, E), k / v -> `cache`
-                   (B, Tmax, 2, E) at slot t0 / *t0_dev
+                   (B, Tmax, 2, E) at slot t0 / *t0_dev; an int8 `cache` with `cache_scale` (B, 2, H, Tmax) fp32 receives
+                   k / v by the int8 KV-cache rule (kv_append_i8)
     rs: `row_scale` (M,) fp32, or rms_from = (partials (M, parts) fp32, eps): rsqrt(mean(x^2) + eps) from a THIN_RES pass."""
     _cuda(x, ACT(), "x"); _cuda(w, ACT(), "w")
     M, K = x.shape
@@ -273,11 +275,11 @@ def linear_thin_fused(x: torch.Tensor, w: torch.Tensor, mode: int, *, row_scale:
     gemm_raw(M=N, N=M, K=Kc, batch=S, A=w.data_ptr(), lda=w.stride(0), a_bs=Kc, B=x.data_ptr(), ldb=x.stride(0), b_bs=Kc,
              Cout=part.data_ptr(), ldc=Mp, c_bs=N * Mp, c_fp32=True, streamk=sk)
     return _thin_tail(part, M, K, mode, row_scale=row_scale, rms_from=rms_from, residual=residual, out=out,
-                      sumsq_out=sumsq_out, rope=rope, cache=cache, t0=t0, t0_dev=t0_dev)
+                      sumsq_out=sumsq_out, rope=rope, cache=cache, t0=t0, t0_dev=t0_dev, cache_scale=cache_scale)
 
 
 def _thin_tail(part: torch.Tensor, M: int, K: int, mode: int, *, row_scale=None, rms_from=None, residual=None, out=None,
-               sumsq_out=None, rope=None, cache=None, t0: int = 0, t0_dev=None) -> torch.Tensor:
+               sumsq_out=None, rope=None, cache=None, t0: int = 0, t0_dev=None, cache_scale=None) -> torch.Tensor:
     """mm_thin_fused over the split-K partial sums part (S, N, Mp) of a thin GEMM with M rows and K columns."""
     S, N, Mp = part.shape
     dev = part.device
@@ -302,12 +304,18 @@ def _thin_tail(part: torch.Tensor, M: int, K: int, mode: int, *, row_scale=None,
         a.sumsq_out = sumsq_out.data_ptr()
     if mode == THIN_QKV:
         cos, sin, pos_dev = rope
-        _cuda(cache, ACT(), "cache")
         E = N // 3
+        if cache_scale is None:
+            _cuda(cache, ACT(), "cache")
+        else:
+            _check_kv_i8(cache, cache_scale, M)
         assert cache.is_contiguous() and cache.dim() == 4 and cache.shape[0] == M and cache.shape[2] == 2 and cache.shape[3] == E
         a.rope_cos, a.rope_sin, a.pos_dev, a.E = cos.data_ptr(), sin.data_ptr(), _ptr(pos_dev), E
         a.cache, a.Tmax, a.t0, a.t0_dev = cache.data_ptr(), cache.shape[1], int(t0), _ptr(t0_dev)
-    _check(_lib.load().mm_thin_fused(C.byref(a), _stream()), "mm_thin_fused")
+    if cache_scale is None:
+        _check(_lib.load().mm_thin_fused(C.byref(a), _stream()), "mm_thin_fused")
+    else:
+        _check(_lib.load().mm_thin_fused_kv_i8(C.byref(a), cache_scale.data_ptr(), _stream()), "mm_thin_fused_kv_i8")
     return out
 
 
@@ -721,6 +729,57 @@ def kv_append(qkv: torch.Tensor, B: int, T_new: int, cache: torch.Tensor, t0: in
     assert qkv.shape == (B * T_new, 3 * E) and qkv.stride(1) == 1 and cache.is_contiguous() and cache.shape[2] == 2
     _check(_lib.load().mm_kv_append(qkv.data_ptr(), qkv.stride(0), B, T_new, E, cache.data_ptr(), cache.shape[1], t0,
                                     _ptr(t0_dev), _stream()), "mm_kv_append")
+
+
+# ---------------------------------------------------------------------------------------------------- int8 KV cache
+def _check_kv_i8(cache: torch.Tensor, cache_scale: torch.Tensor, B: int) -> None:
+    """cache int8 (B, Tmax, 2, E) and cache_scale fp32 (B, 2, E / 128, Tmax), both contiguous (mm_kv_append_i8's layout)."""
+    _cuda(cache, torch.int8, "cache"); _cuda(cache_scale, torch.float32, "cache_scale")
+    assert cache.dim() == 4 and cache.is_contiguous() and cache.shape[0] == B and cache.shape[2] == 2, cache.shape
+    _, Tmax, _, E = cache.shape
+    assert tuple(cache_scale.shape) == (B, 2, E // 128, Tmax) and cache_scale.is_contiguous(), cache_scale.shape
+
+
+def kv_append_i8(qkv: torch.Tensor, B: int, T_new: int, cache: torch.Tensor, cache_scale: torch.Tensor, t0: int,
+                 t0_dev: Optional[torch.Tensor] = None) -> None:
+    """`kv_append` into an int8 cache: each k / v head vector of the rows (16-bit, as the 16-bit cache stores it) is
+    quantized by the int8 KV-cache rule (mm_kv_append_i8): s = fp32(max |v|) / 127, q = clamp(rint(v / s), -127, 127),
+    q = 0 where s = 0; q -> cache (B, Tmax, 2, E), s -> cache_scale (B, 2, H, Tmax)."""
+    _cuda(qkv, ACT(), "qkv")
+    _check_kv_i8(cache, cache_scale, B)
+    E = cache.shape[-1]
+    assert qkv.shape == (B * T_new, 3 * E) and qkv.stride(1) == 1
+    _check(_lib.load().mm_kv_append_i8(qkv.data_ptr(), qkv.stride(0), B, T_new, E, cache.data_ptr(), cache_scale.data_ptr(),
+                                       cache.shape[1], t0, _ptr(t0_dev), _stream()), "mm_kv_append_i8")
+
+
+def attention_decode_i8(q: torch.Tensor, cache: torch.Tensor, cache_scale: torch.Tensor, *, scale: float,
+                        Tk: Optional[int] = None, tk_dev: Optional[torch.Tensor] = None,
+                        key_mask: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Attention of one query row per (sample, head) over an int8 cache (mm_attn_decode_i8): q (B, 1, H, 128) 16-bit view
+    (head_dim contiguous, heads 128 apart), cache / cache_scale as kv_append_i8 fills them -> (B, 1, H, 128).  The key count
+    is Tk (default: the capacity), or min(*tk_dev, Tk) read on the device.  There is no key mask: generate never passes one."""
+    if key_mask is not None:
+        raise NotImplementedError("macaw_b200: the int8 KV cache's decode attention takes no key mask")
+    _cuda(q, ACT(), "q")
+    B, Tq, H, hd = q.shape
+    assert Tq == 1 and hd == 128 and q.stride(3) == 1 and q.stride(2) == 128, (q.shape, q.stride())
+    _check_kv_i8(cache, cache_scale, B)
+    Tmax = cache.shape[1]
+    assert cache.shape[3] == H * hd
+    Tk = Tmax if Tk is None else int(Tk)
+    if tk_dev is not None:
+        _cuda(tk_dev, torch.int32, "tk_dev")
+    if out is None:
+        out = torch.empty((B, 1, H, hd), device=q.device, dtype=ACT())
+    assert out.shape == (B, 1, H, hd) and out.stride(3) == 1 and out.stride(2) == 128
+    lib = _lib.load()
+    nbytes = int(lib.mm_attn_decode_i8_workspace_bytes(B, H, Tmax))
+    ws = torch.empty(((nbytes + 15) // 16 * 4,), device=q.device, dtype=torch.float32)
+    _check(lib.mm_attn_decode_i8(q.data_ptr(), q.stride(0), cache.data_ptr(), cache_scale.data_ptr(), out.data_ptr(),
+                                 out.stride(0), B, H, Tmax, Tk, _ptr(tk_dev), float(scale), ws.data_ptr(), ws.numel() * 4,
+                                 _stream()), "mm_attn_decode_i8")
+    return out
 
 
 def rope_rows(x: torch.Tensor, rot_cols: int, cos: torch.Tensor, sin: torch.Tensor, rope_T: int,

@@ -11,7 +11,16 @@ otherwise: peak device memory of each (measured with only that model's working s
 prefill ms and decode ms/step at B = 1, 8, 64 and two at B = 96, then each decode GEMM with its tail alone (one call per
 layer captured in a CUDA graph and replayed between CUDA events, so no host time is counted and, with the weights of all
 32 layers in turn, nothing is served from L2): the 16-bit linear_thin_fused against the int8 linear_w8_thin_fused at
-M = 1, 8, 64, with the weight bytes each streams per second as a share of 3.35 TB/s."""
+M = 1, 8, 64, with the weight bytes each streams per second as a share of 3.35 TB/s.
+
+--kv-int8: the 16-bit KV cache against the int8 one (Engine.enable_int8_kv_cache), bf16 unless --dtype says otherwise.
+First the decode attention alone: ops.attention (fa_wgmma_kernel at Tq = 1) over 16-bit caches against
+ops.attention_decode_i8 over int8 caches, one call per layer over 32 layers' caches captured in a CUDA graph and replayed
+between CUDA events (nothing served from L2), at Tk = 264 of 320 rows for B = 1, 8, 64, 96 and Tk = 2048 of 2112 at B = 8,
+with the cache bytes each reads per second as a share of 3.35 TB/s.  Then generate() with 16-bit and with int8 decoder
+weights: per weight format, the peak device memory of a B = 64 call with each cache, and three alternated rounds of
+prefill ms and decode ms/step at T = 264, B = 1, 8, 64, 96, and at T = 2048, B = 8 (two engines on one model, sharing its
+derived weights, so that neither re-captures its decode graph between rounds)."""
 import argparse
 import os
 import subprocess
@@ -176,6 +185,79 @@ def _int8(a, cfg, dtype):
                   f"{b8 / t8 / 1e6 / HBM_BPS * 1e12:.0%}); {t16 / t8:.2f}x")
 
 
+def _kv_int8(a, cfg, dtype):
+    from macaw_llm_b200 import ops
+    from macaw_llm_b200.engine import Engine, KVCacheInt8
+    from macaw_llm_b200.modeling import MM_LLMs
+
+    llama = cfg.llm_config
+    E, Hh, L = llama.hidden_size, llama.num_attention_heads, llama.num_hidden_layers
+    print(f"[bench_decode] {_card()}; 16-bit vs int8 KV cache, {dtype}")
+    ops.set_act_format(dtype)
+    scale = 128 ** -0.5
+    for B, tk, t_max in ((1, 264, 320), (8, 264, 320), (64, 264, 320), (96, 264, 320), (8, 2048, 2112)):
+        g = torch.Generator(device="cuda").manual_seed(B + tk)
+        q = torch.randn((B, 1, Hh, 128), device="cuda", generator=g).to(dtype)
+        c16 = [torch.randn((B, t_max, 2, E), device="cuda", generator=g).to(dtype) for _ in range(L)]
+        c8 = KVCacheInt8.allocate(B, t_max, L, E, "cuda")
+        qkv = torch.empty((B, 3 * E), device="cuda", dtype=dtype)
+        for i in range(L):
+            for t in range(0, t_max, 64):  # the int8 caches hold the quantized 16-bit ones
+                qkv.view(B, 3, E)[:, 1:] = c16[i][:, t]
+                ops.kv_append_i8(qkv, B, 1, c8.layers[i], c8.ks[i], t)
+        tk_dev = torch.tensor([tk], device="cuda", dtype=torch.int32)
+        kv = [c.unflatten(-1, (Hh, 128)) for c in c16]
+        t16 = _gemm_us(lambda i: ops.attention(q, kv[i][:, :, 0], kv[i][:, :, 1], scale=scale, tk_dev=tk_dev), L, 20)
+        t8 = _gemm_us(lambda i: ops.attention_decode_i8(q, c8.layers[i], c8.ks[i], scale=scale, tk_dev=tk_dev), L, 20)
+        b16, b8 = B * Hh * tk * 2 * 128 * 2, B * Hh * tk * 2 * (128 + 4)
+        print(f"[bench_decode] attention B={B:2d} Tk={tk} of {t_max}: 16-bit fa_wgmma {t16:7.1f} us "
+              f"({b16 / t16 / 1e6:.2f} TB/s, {b16 / t16 / 1e6 / HBM_BPS * 1e12:.0%}); int8 decode {t8:7.1f} us "
+              f"({b8 / t8 / 1e6:.2f} TB/s, {b8 / t8 / 1e6 / HBM_BPS * 1e12:.0%}); {t16 / t8:.2f}x")
+        del c16, c8, kv
+        torch.cuda.empty_cache()
+
+    def inputs(B, seq_len):
+        host = bench.synth_inputs(B, seq_len, llama.vocab_size, 224, 3000, 1234)
+        host["audios"] = None
+        return {k: (v.cuda() if isinstance(v, torch.Tensor) else v) for k, v in host.items()}
+
+    for wname in ("16-bit", "int8"):
+        m = MM_LLMs.build_random(cfg, device="cuda", dtype=dtype, seed=0)
+        if wname == "int8":
+            m.quantize_llm_int8()
+        engs = {"16-bit cache": m.engine, "int8 cache": Engine(m)}
+        engs["int8 cache"]._cache = m.engine._cache  # the derived weights are the same: keep one copy
+        engs["int8 cache"].enable_int8_kv_cache(True)
+        inp = inputs(64, a.seq_len)
+        for name, eng in engs.items():
+            eng.generate(inp, max_new_tokens=a.new, eos_token_id=-1)
+            eng._decode.clear()
+            torch.cuda.synchronize()
+            torch.cuda.empty_cache()
+            base = torch.cuda.memory_allocated()
+            torch.cuda.reset_peak_memory_stats()
+            eng.generate(inp, max_new_tokens=a.new, eos_token_id=-1)
+            torch.cuda.synchronize()
+            peak = torch.cuda.max_memory_allocated() - base
+            print(f"[bench_decode] {wname} weights, {name}: peak memory of a B = 64, T = {a.seq_len + 8}, "
+                  f"new = {a.new} call above the resident model: {peak / 2 ** 30:.2f} GiB")
+            eng._decode.clear()
+        for B, seq_len in ((1, a.seq_len), (8, a.seq_len), (64, a.seq_len), (96, a.seq_len), (8, 2040)):
+            inp = inputs(B, seq_len)
+            for eng in engs.values():  # warm-up: KV caches and the decode graph of this shape
+                eng.generate(inp, max_new_tokens=a.new, eos_token_id=-1)
+            for rnd in range(3):
+                res = {name: _decode_ms(eng, inp, a.new) for name, eng in engs.items()}
+                print(f"[bench_decode] {wname} weights round {rnd} B={B:2d} T={seq_len + 8}: " + "; ".join(
+                    f"{n} prefill {p:.1f} ms, decode {st:.3f} ms/step" for n, (p, st) in res.items()))
+            for eng in engs.values():
+                eng._decode.clear()
+            del inp
+            torch.cuda.empty_cache()
+        del engs, m
+        torch.cuda.empty_cache()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=8)
@@ -187,6 +269,7 @@ def main():
     ap.add_argument("--top-p", type=float, default=0.6)
     ap.add_argument("--repetition-penalty", type=float, default=1.0)
     ap.add_argument("--int8", action="store_true", help="compare the 16-bit decoder with its int8-quantized twin")
+    ap.add_argument("--kv-int8", action="store_true", help="compare the 16-bit KV cache with the int8 one")
     ap.add_argument("--dtype", choices=("bf16", "fp16"), default=None, help="default: fp16 with --sample / --int8, else bf16")
     a = ap.parse_args()
     from macaw_llm_b200 import ops
@@ -197,6 +280,8 @@ def main():
     cfg = MM_LLMs_Config(clip_config=clip, whisper_config=whisper, llm_config=llama, **hyper)
     if a.int8:
         return _int8(a, cfg, dtype)
+    if a.kv_int8:
+        return _kv_int8(a, cfg, dtype)
     model = MM_LLMs.build_random(cfg, device="cuda", dtype=dtype, seed=0)
     host = bench.synth_inputs(a.batch, a.seq_len, llama.vocab_size, 224, 3000, 1234)
     host["audios"] = None
